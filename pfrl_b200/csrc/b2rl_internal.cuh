@@ -117,11 +117,29 @@ int b2rl_stage_release(b2rl_replay *h, cudaStream_t s);
 static constexpr unsigned B2RL_N_TICKETS = 256;
 unsigned b2rl_next_ticket();
 
-// exact sampler generation for a tree of this depth (sampler.cu; env B2RL_SAMPLER=v5)
-bool b2rl_use_v6(int levels);
-int b2rl_v6_slow_every();
-double b2rl_v6_eps_scale();
-int b2rl_v6_sleep_scale();
+// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device)
+template <auto KERNEL>
+static cudaError_t b2rl_allow_smem(size_t bytes)
+{
+    static bool done[64];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    if (dev < 0 || dev >= 64 || !done[dev]) {
+        e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+        if (e != cudaSuccess) return e;
+        if (dev >= 0 && dev < 64) done[dev] = true;
+    }
+    return cudaSuccess;
+}
+
+// Sampler arguments of a draw of n uniforms `u` (device) from the handle's trees: the
+// shared-memory split (T, D), the handle's slot / priority outputs, the optional user
+// outputs and the exact sampler's test hooks (env B2RL_V6_SLOW_EVERY / B2RL_V6_EPS_SCALE);
+// no weights, no publication to other CTAs (sampler.cu, SampleArgs: tree_dev.cuh).
+struct SampleArgs;
+SampleArgs b2rl_sample_args(const b2rl_replay *h, const double *u, int n, int64_t *index_out,
+                            double *prio_user);
 
 // Apply a write-back registered with b2rl_per_defer_errors (no-op if none).
 int b2rl_flush_pending(b2rl_replay *h, cudaStream_t s);

@@ -21,7 +21,7 @@
 #include <atomic>
 #include <new>
 
-#include "b2rl_internal.cuh"
+#include "tree_dev.cuh"
 
 // ---------------------------------------------------------------------------
 static thread_local char g_err[512] = "";
@@ -168,31 +168,8 @@ __global__ void __launch_bounds__(1024) k_tree_fix_small(FixArgs a)
         }
         __syncthreads();
     }
-    // ... then the top `topl` levels (<= 1023 nodes) entirely in shared memory:
-    // nodes are pure functions of their children, so recomputing all of them
-    // from level `topl` is exact and saves ten global round trips
-    if (a.nranges > 0) {
-        __shared__ double s_sum[2048], s_min[2048];
-        const int base = 1 << topl;
-        for (int i = threadIdx.x; i < base; i += blockDim.x) {
-            s_sum[base + i] = a.sum[base + i];
-            s_min[base + i] = a.mn[base + i];
-        }
-        __syncthreads();
-        for (int lv = topl - 1; lv >= 0; lv--) {
-            const int w = 1 << lv;
-            for (int i = threadIdx.x; i < w; i += blockDim.x) {
-                const int node = w + i;
-                s_sum[node] = s_sum[2 * node] + s_sum[2 * node + 1];
-                s_min[node] = fmin(s_min[2 * node], s_min[2 * node + 1]);
-            }
-            __syncthreads();
-        }
-        for (int i = 1 + threadIdx.x; i < base; i += blockDim.x) {
-            a.sum[i] = s_sum[i];
-            a.mn[i] = s_min[i];
-        }
-    }
+    // ... then the top `topl` levels entirely in shared memory
+    if (a.nranges > 0) rebuild_top_levels(a.sum, a.mn, topl);
     if (threadIdx.x == 0 && a.bump_n > 0) {
         long long napp = a.st->napp + a.bump_n;
         long long npop = a.st->npop;
@@ -405,13 +382,7 @@ int b2rl_launch_tree_fix(b2rl_replay *h, int nranges, long long *lo, long long *
             cnt[r] = hi[r] - lo[r] + 1;
             total += cnt[r];
         }
-        static int level_sync = -1; // B2RL_REPAIR=levels keeps the old kernels
-        if (level_sync < 0) {
-            const char *e = getenv("B2RL_REPAIR");
-            level_sync = (e && e[0] == 'l') ? 1 : 0;
-        }
-        if (total <= 512 && !level_sync)
-            return b2rl_launch_repair_multi(h, nranges, first, cnt, bump_n, s);
+        if (total <= UPD_MAX) return b2rl_launch_repair_multi(h, nranges, first, cnt, bump_n, s);
     }
     int level = h->levels; // lo/hi are leaf-level node indices
     if (h->cfg.prioritized) {

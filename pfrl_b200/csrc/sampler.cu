@@ -37,10 +37,17 @@ __global__ void __launch_bounds__(256, 1) k_sample_exact(SampleArgs a)
 }
 
 // main warp + two scouts + publisher (tree_dev.cuh)
-template <int D, bool FMA>
+template <int D>
 __global__ void __launch_bounds__(128, 1) k_sample_exact_deep(SampleArgs a)
 {
-    exact_deep<D, FMA>(a, reinterpret_cast<double *>(smem_raw));
+    exact_deep<D>(a, reinterpret_cast<double *>(smem_raw));
+}
+
+// v6 (tree_dev.cuh): decisions on an approximate top, exact re-reduction on a trailing warp
+template <int D>
+__global__ void __launch_bounds__(V6_THREADS, 1) k_sample_exact_v6(SampleArgs a)
+{
+    exact_deep_v6<D>(a, reinterpret_cast<double *>(smem_raw));
 }
 
 __global__ void __launch_bounds__(512, 1) k_sample_parallel(SampleArgs a)
@@ -48,79 +55,41 @@ __global__ void __launch_bounds__(512, 1) k_sample_parallel(SampleArgs a)
     sample_parallel(a, reinterpret_cast<double *>(smem_raw));
 }
 
-// cudaFuncSetAttribute once per (kernel, device)
-template <typename K>
-static cudaError_t allow_smem(K kernel, size_t bytes, bool *done_per_device)
+static cudaError_t launch_sample(const SampleArgs &a, int mode, cudaStream_t s)
 {
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    if (dev < 0 || dev >= 64 || !done_per_device[dev]) {
-        e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    const SamplerChoice c = choose_sampler(mode, a.levels, a.n);
+    switch (c.kind) {
+    case SAMPLER_V6:
+        return with_depth<5, 9>(c.D, [&](auto d) {
+            constexpr int D = decltype(d)::value;
+            const size_t smem = exact_v6_smem_bytes<D>();
+            const cudaError_t e = b2rl_allow_smem<k_sample_exact_v6<D>>(smem);
+            if (e != cudaSuccess) return e;
+            k_sample_exact_v6<D><<<1, V6_THREADS, smem, s>>>(a);
+            return cudaGetLastError();
+        });
+    case SAMPLER_V5:
+        return with_depth<1, 10>(c.D, [&](auto d) {
+            constexpr int D = decltype(d)::value;
+            const size_t smem = exact_deep_smem_bytes<D>();
+            const cudaError_t e = b2rl_allow_smem<k_sample_exact_deep<D>>(smem);
+            if (e != cudaSuccess) return e;
+            k_sample_exact_deep<D><<<1, 128, smem, s>>>(a);
+            return cudaGetLastError();
+        });
+    case SAMPLER_SMALL: {
+        const cudaError_t e = b2rl_allow_smem<k_sample_exact>(200 * 1024);
         if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < 64) done_per_device[dev] = true;
+        k_sample_exact<<<1, 256, sizeof(double) * ((size_t(1) << a.T) + (size_t(2) << a.D)), s>>>(a);
+        return cudaGetLastError();
     }
-    return cudaSuccess;
-}
-
-template <int D, bool FMA>
-static cudaError_t launch_deep_as(const SampleArgs &a, cudaStream_t s)
-{
-    const size_t smem = exact_deep_smem_bytes<D>();
-    static bool done[64];
-    cudaError_t e = allow_smem(k_sample_exact_deep<D, FMA>, smem, done);
-    if (e != cudaSuccess) return e;
-    k_sample_exact_deep<D, FMA><<<1, 128, smem, s>>>(a);
-    return cudaGetLastError();
-}
-
-static bool fma_descent_requested()
-{
-    static int cached = -1;
-    if (cached < 0) {
-        const char *e = getenv("B2RL_SAMPLER_DESCENT");
-        cached = (e && e[0] == 's') ? 0 : 1;
+    default:
+        k_sample_parallel<<<1, 512, 64 * sizeof(double), s>>>(a);
+        return cudaGetLastError();
     }
-    return cached == 1;
 }
 
-template <int D>
-static cudaError_t launch_deep(const SampleArgs &a, cudaStream_t s)
-{
-    return fma_descent_requested() ? launch_deep_as<D, true>(a, s)
-                                   : launch_deep_as<D, false>(a, s);
-}
-
-// v6 (tree_dev.cuh): decisions on an approximate top, exact re-reduction on a trailing warp
-template <int D>
-__global__ void __launch_bounds__(V6_THREADS, 1) k_sample_exact_v6(SampleArgs a)
-{
-    exact_deep_v6<D, true>(a, reinterpret_cast<double *>(smem_raw));
-}
-
-template <int D>
-static cudaError_t launch_v6_as(const SampleArgs &a, cudaStream_t s)
-{
-    const size_t smem = exact_v6_smem_bytes<D>();
-    static bool done[64];
-    cudaError_t e = allow_smem(k_sample_exact_v6<D>, smem, done);
-    if (e != cudaSuccess) return e;
-    k_sample_exact_v6<D><<<1, V6_THREADS, smem, s>>>(a);
-    return cudaGetLastError();
-}
-
-// B2RL_SAMPLER=v5 keeps the single-chain sampler for trees v6 covers (levels 17..21)
-bool b2rl_use_v6(int levels)
-{
-    static int cached = -1;
-    if (cached < 0) {
-        const char *e = getenv("B2RL_SAMPLER");
-        cached = (e && e[0] == 'v' && e[1] == '5') ? 0 : 1;
-    }
-    return cached == 1 && levels >= 17 && levels <= 21; // v6 stages 5..9 levels per draw
-}
-
-int b2rl_v6_slow_every()
+static int v6_slow_every()
 {
     static int cached = -1;
     if (cached < 0) {
@@ -131,18 +100,7 @@ int b2rl_v6_slow_every()
     return cached;
 }
 
-int b2rl_v6_sleep_scale()
-{
-    static int cached = -1;
-    if (cached < 0) {
-        const char *e = getenv("B2RL_V6_SLEEP");
-        cached = e ? atoi(e) : 1;
-        if (cached < 1) cached = 1;
-    }
-    return cached;
-}
-
-double b2rl_v6_eps_scale()
+static double v6_eps_scale()
 {
     static double cached = -1.0;
     if (cached < 0.0) {
@@ -153,34 +111,27 @@ double b2rl_v6_eps_scale()
     return cached;
 }
 
-static cudaError_t launch_exact_v6(const SampleArgs &a, cudaStream_t s)
+SampleArgs b2rl_sample_args(const b2rl_replay *h, const double *u, int n, int64_t *index_out,
+                            double *prio_user)
 {
-    switch (a.levels - (V6_T - 1)) {
-    case 5: return launch_v6_as<5>(a, s);
-    case 6: return launch_v6_as<6>(a, s);
-    case 7: return launch_v6_as<7>(a, s);
-    case 8: return launch_v6_as<8>(a, s);
-    case 9: return launch_v6_as<9>(a, s);
-    default: return cudaErrorInvalidValue;
-    }
-}
-
-static cudaError_t launch_exact_deep(const SampleArgs &a, cudaStream_t s)
-{
-    if (b2rl_use_v6(a.levels) && a.n <= 60000) return launch_exact_v6(a, s); // u16 draw ids
-    switch (a.D) {
-    case 1: return launch_deep<1>(a, s);
-    case 2: return launch_deep<2>(a, s);
-    case 3: return launch_deep<3>(a, s);
-    case 4: return launch_deep<4>(a, s);
-    case 5: return launch_deep<5>(a, s);
-    case 6: return launch_deep<6>(a, s);
-    case 7: return launch_deep<7>(a, s);
-    case 8: return launch_deep<8>(a, s);
-    case 9: return launch_deep<9>(a, s);
-    case 10: return launch_deep<10>(a, s);
-    default: return cudaErrorInvalidValue;
-    }
+    SampleArgs a{};
+    a.sum = h->sum;
+    a.mn = h->mn;
+    a.st = h->st;
+    a.u = u;
+    a.n = n;
+    a.levels = h->levels;
+    a.nslots = h->nslots;
+    a.T = h->levels + 1 < TOP_LEVELS ? h->levels + 1 : TOP_LEVELS;
+    a.D = h->levels - (a.T - 1);
+    a.slots_out = h->last_slots;
+    a.prio_out = h->last_prio;
+    a.index_out = (long long *)index_out;
+    a.prio_user = prio_user;
+    a.norm = B2RL_NORM_NONE;
+    a.dbg_slow_every = v6_slow_every();
+    a.dbg_eps_scale = v6_eps_scale();
+    return a;
 }
 
 extern "C" int b2rl_per_sample(b2rl_replay *h, const double *u_host, int32_t n, int mode,
@@ -209,41 +160,8 @@ extern "C" int b2rl_per_sample(b2rl_replay *h, const double *u_host, int32_t n, 
     B2RL_CUDA(cudaMemcpyAsync(h->u_dev, h->pin, (size_t)n * 8, cudaMemcpyHostToDevice, s));
     TRY(b2rl_stage_release(h, s));
 
-    SampleArgs a;
-    a.sum = h->sum;
-    a.mn = h->mn;
-    a.st = h->st;
-    a.u = h->u_dev;
-    a.n = n;
-    a.levels = h->levels;
-    a.nslots = h->nslots;
-    a.T = h->levels + 1 < TOP_LEVELS ? h->levels + 1 : TOP_LEVELS;
-    a.D = h->levels - (a.T - 1);
-    a.slots_out = h->last_slots;
-    a.prio_out = h->last_prio;
-    a.index_out = (long long *)index_dev;
-    a.prio_user = priority_dev;
-    a.weight = nullptr; // weights are a separate call on this path (b2rl_per_weights)
-    a.prob = nullptr;
-    a.beta = 0.0;
-    a.norm = B2RL_NORM_NONE;
-    a.ready = nullptr;
-    a.seq_base = 0;
-    a.dbg_slow_every = b2rl_v6_slow_every();
-    a.dbg_eps_scale = b2rl_v6_eps_scale();
-    a.dbg_sleep_scale = b2rl_v6_sleep_scale();
-    a.dbg_cycles = nullptr;
-    if (mode == B2RL_SAMPLE_EXACT && a.D > 0) {
-        B2RL_CUDA(launch_exact_deep(a, s));
-    } else if (mode == B2RL_SAMPLE_EXACT) {
-        size_t smem = sizeof(double) * ((size_t(1) << a.T) + (size_t(2) << a.D));
-        static bool done[64];
-        B2RL_CUDA(allow_smem(k_sample_exact, 200 * 1024, done));
-        k_sample_exact<<<1, 256, smem, s>>>(a);
-    } else {
-        k_sample_parallel<<<1, 512, 64 * sizeof(double), s>>>(a);
-    }
-    B2RL_CUDA(cudaGetLastError());
+    // weights are a separate call on this path (b2rl_per_weights)
+    B2RL_CUDA(launch_sample(b2rl_sample_args(h, h->u_dev, n, index_dev, priority_dev), mode, s));
     h->wait_priority = true;
     h->last_n = n;
     h->last_mode = mode;
@@ -316,18 +234,23 @@ extern "C" int b2rl_per_weights(b2rl_replay *h, double beta, int norm, float *we
 // ---------------------------------------------------------------------------
 // priority write-back
 // ---------------------------------------------------------------------------
-// UpdateArgs, tree_update_paths(): tree_dev.cuh.  n <= UPD_MAX takes the sorted-path
+// UpdateArgs, tree_update_multi(): tree_dev.cuh.  n <= UPD_MAX takes the sorted-path
 // kernel (one global round trip); larger batches the level-synchronous one below.
-__global__ void __launch_bounds__(512, 1) k_update_paths(UpdateArgs a)
-{
-    tree_update_paths(a, smem_raw);
-}
-
-// one CTA per subtree below level 7, the last one to arrive finishes the top
+// One CTA per subtree below level 7, the last one to arrive finishes the top.
 __global__ void __launch_bounds__(256) k_update_multi(UpdateArgs a, unsigned long long *sync,
                                                       unsigned long long seq)
 {
     tree_update_multi(a, smem_raw, sync, seq);
+}
+
+static int launch_update_multi(b2rl_replay *h, const UpdateArgs &a, cudaStream_t s)
+{
+    B2RL_CUDA(b2rl_allow_smem<k_update_multi>(227 * 1024)); // once per device: the maximum
+    const int grid = 1 << update_split_level(h->levels);
+    k_update_multi<<<grid, 256, update_multi_smem_bytes(h->levels), s>>>(
+        a, h->ready_dev + 1, (unsigned long long)h->step_seq << 32);
+    B2RL_CUDA(cudaGetLastError());
+    return B2RL_OK;
 }
 
 __global__ void __launch_bounds__(1024) k_update(UpdateArgs a)
@@ -392,31 +315,7 @@ __global__ void __launch_bounds__(1024) k_update(UpdateArgs a)
             __syncthreads();
         }
     }
-    // top `topl` levels (<= 1023 nodes per tree): every node is a pure function
-    // of its children, so recompute them all from level `topl` in shared memory
-    // (cheap barriers) instead of ten more global round trips
-    {
-        __shared__ double s_sum[2048], s_min[2048];
-        const int base = 1 << topl;
-        for (int i = tid; i < base; i += nt) {
-            s_sum[base + i] = a.sum[base + i];
-            s_min[base + i] = a.mn[base + i];
-        }
-        __syncthreads();
-        for (int lv = topl - 1; lv >= 0; lv--) {
-            const int w = 1 << lv;
-            for (int i = tid; i < w; i += nt) {
-                const int node = w + i;
-                s_sum[node] = s_sum[2 * node] + s_sum[2 * node + 1];
-                s_min[node] = fmin(s_min[2 * node], s_min[2 * node + 1]);
-            }
-            __syncthreads();
-        }
-        for (int i = 1 + tid; i < base; i += nt) {
-            a.sum[i] = s_sum[i];
-            a.mn[i] = s_min[i];
-        }
-    }
+    rebuild_top_levels(a.sum, a.mn, topl);
     for (int k = tid; k < a.n; k += nt) a.winner[a.slots[k]] = -1;
     for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
     if ((tid & 31) == 0) red[tid >> 5] = mx;
@@ -454,27 +353,12 @@ static int launch_update(b2rl_replay *h, int32_t n, const void *err, int err_is_
     a.bump_n = 0;
     a.capacity = h->cfg.capacity;
     a.stamps = nullptr;
-    static int single_cta = -1; // B2RL_UPDATE=single keeps the one-CTA sorted-path kernel
-    if (single_cta < 0) {
-        const char *e = getenv("B2RL_UPDATE");
-        single_cta = (e && e[0] == 's') ? 1 : 0;
-    }
-    if (n <= UPD_MAX && !single_cta) {
-        const size_t smem = update_multi_smem_bytes(h->levels);
-        static bool done[64];
-        B2RL_CUDA(allow_smem(k_update_multi, 227 * 1024, done)); // once per device: the maximum
-        const int grid = 1 << update_split_level(h->levels);
-        k_update_multi<<<grid, 256, smem, s>>>(a, h->ready_dev + 1,
-                                               (unsigned long long)h->step_seq << 32);
-    } else if (n <= UPD_MAX) {
-        const size_t smem = update_paths_smem_bytes(h->levels);
-        static bool done[64];
-        B2RL_CUDA(allow_smem(k_update_paths, 227 * 1024, done));
-        k_update_paths<<<1, 512, smem, s>>>(a);
+    if (n <= UPD_MAX) {
+        TRY(launch_update_multi(h, a, s));
     } else {
         k_update<<<1, 1024, 0, s>>>(a);
+        B2RL_CUDA(cudaGetLastError());
     }
-    B2RL_CUDA(cudaGetLastError());
     h->wait_priority = false;
     h->last_n = 0;
     return B2RL_OK;
@@ -545,14 +429,7 @@ int b2rl_launch_repair_multi(b2rl_replay *h, int nranges, const long long *first
     a.n = total;
     a.bump_n = bump_n;
     a.capacity = h->cfg.capacity;
-    const size_t smem = update_multi_smem_bytes(h->levels);
-    static bool done[64];
-    B2RL_CUDA(allow_smem(k_update_multi, 227 * 1024, done));
-    const int grid = 1 << update_split_level(h->levels);
-    k_update_multi<<<grid, 256, smem, s>>>(a, h->ready_dev + 1,
-                                           (unsigned long long)h->step_seq << 32);
-    B2RL_CUDA(cudaGetLastError());
-    return B2RL_OK;
+    return launch_update_multi(h, a, s);
 }
 
 // Deferred form: register the TD errors of the last sample; the trees are

@@ -260,8 +260,7 @@ __device__ __forceinline__ void gather_worker(const StepGather &g, unsigned char
     }
 }
 
-// MODE 0: exact v5, deep tree (template D = levels - 13); 1: exact, tree in shared memory;
-// 2: parallel; 3: exact v6 (template D = levels - 12)
+// MODE: the SamplerKind of choose_sampler (tree_dev.cuh), D its template depth
 template <int D, int MODE>
 __global__ void __launch_bounds__(STEP_THREADS, 1) k_replay_step(const __grid_constant__ StepArgs a)
 {
@@ -278,11 +277,11 @@ __global__ void __launch_bounds__(STEP_THREADS, 1) k_replay_step(const __grid_co
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) a.times[1] = global_ns();
     if (blockIdx.x == 0) {
-        if constexpr (MODE == 0)
-            exact_deep<D, true>(a.s, reinterpret_cast<double *>(smem_raw));
-        else if constexpr (MODE == 3)
-            exact_deep_v6<D, true>(a.s, reinterpret_cast<double *>(smem_raw));
-        else if constexpr (MODE == 1)
+        if constexpr (MODE == SAMPLER_V5)
+            exact_deep<D>(a.s, reinterpret_cast<double *>(smem_raw));
+        else if constexpr (MODE == SAMPLER_V6)
+            exact_deep_v6<D>(a.s, reinterpret_cast<double *>(smem_raw));
+        else if constexpr (MODE == SAMPLER_SMALL)
             exact_small(a.s, reinterpret_cast<double *>(smem_raw));
         else
             sample_parallel(a.s, reinterpret_cast<double *>(smem_raw));
@@ -297,57 +296,34 @@ __global__ void __launch_bounds__(STEP_THREADS, 1) k_replay_step(const __grid_co
 template <int D, int MODE>
 static cudaError_t launch_step_as(const StepArgs &a, int grid, size_t smem, cudaStream_t s)
 {
-    static bool done[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
+    const cudaError_t e = b2rl_allow_smem<k_replay_step<D, MODE>>(227 * 1024);
     if (e != cudaSuccess) return e;
-    if (dev < 0 || dev >= 64 || !done[dev]) {
-        e = cudaFuncSetAttribute(k_replay_step<D, MODE>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < 64) done[dev] = true;
-    }
     k_replay_step<D, MODE><<<grid, STEP_THREADS, smem, s>>>(a);
     return cudaGetLastError();
-}
-
-template <int D>
-static size_t deep_bytes()
-{
-    return exact_deep_smem_bytes<D>();
 }
 
 static cudaError_t launch_step(const StepArgs &a, int mode, int grid, size_t smem_other,
                                cudaStream_t s)
 {
     auto mx = [](size_t x, size_t y) { return x > y ? x : y; };
-    if (mode == B2RL_SAMPLE_PARALLEL) return launch_step_as<0, 2>(a, grid, mx(smem_other, 1024), s);
-    if (a.s.D == 0) {
+    const SamplerChoice c = choose_sampler(mode, a.s.levels, a.s.n);
+    switch (c.kind) {
+    case SAMPLER_PARALLEL:
+        return launch_step_as<0, SAMPLER_PARALLEL>(a, grid, mx(smem_other, 1024), s);
+    case SAMPLER_SMALL: {
         const size_t sm = sizeof(double) * ((size_t(1) << a.s.T) + 2);
-        return launch_step_as<0, 1>(a, grid, mx(smem_other, sm), s);
+        return launch_step_as<0, SAMPLER_SMALL>(a, grid, mx(smem_other, sm), s);
     }
-    if (b2rl_use_v6(a.s.levels) && a.s.n <= 60000) {
-        switch (a.s.levels - (V6_T - 1)) {
-        case 5: return launch_step_as<5, 3>(a, grid, mx(smem_other, exact_v6_smem_bytes<5>()), s);
-        case 6: return launch_step_as<6, 3>(a, grid, mx(smem_other, exact_v6_smem_bytes<6>()), s);
-        case 7: return launch_step_as<7, 3>(a, grid, mx(smem_other, exact_v6_smem_bytes<7>()), s);
-        case 8: return launch_step_as<8, 3>(a, grid, mx(smem_other, exact_v6_smem_bytes<8>()), s);
-        case 9: return launch_step_as<9, 3>(a, grid, mx(smem_other, exact_v6_smem_bytes<9>()), s);
-        default: return cudaErrorInvalidValue;
-        }
-    }
-    switch (a.s.D) {
-    case 1: return launch_step_as<1, 0>(a, grid, mx(smem_other, deep_bytes<1>()), s);
-    case 2: return launch_step_as<2, 0>(a, grid, mx(smem_other, deep_bytes<2>()), s);
-    case 3: return launch_step_as<3, 0>(a, grid, mx(smem_other, deep_bytes<3>()), s);
-    case 4: return launch_step_as<4, 0>(a, grid, mx(smem_other, deep_bytes<4>()), s);
-    case 5: return launch_step_as<5, 0>(a, grid, mx(smem_other, deep_bytes<5>()), s);
-    case 6: return launch_step_as<6, 0>(a, grid, mx(smem_other, deep_bytes<6>()), s);
-    case 7: return launch_step_as<7, 0>(a, grid, mx(smem_other, deep_bytes<7>()), s);
-    case 8: return launch_step_as<8, 0>(a, grid, mx(smem_other, deep_bytes<8>()), s);
-    case 9: return launch_step_as<9, 0>(a, grid, mx(smem_other, deep_bytes<9>()), s);
-    case 10: return launch_step_as<10, 0>(a, grid, mx(smem_other, deep_bytes<10>()), s);
-    default: return cudaErrorInvalidValue;
+    case SAMPLER_V6:
+        return with_depth<5, 9>(c.D, [&](auto d) {
+            constexpr int D = decltype(d)::value;
+            return launch_step_as<D, SAMPLER_V6>(a, grid, mx(smem_other, exact_v6_smem_bytes<D>()), s);
+        });
+    default:
+        return with_depth<1, 10>(c.D, [&](auto d) {
+            constexpr int D = decltype(d)::value;
+            return launch_step_as<D, SAMPLER_V5>(a, grid, mx(smem_other, exact_deep_smem_bytes<D>()), s);
+        });
     }
 }
 
@@ -419,28 +395,13 @@ extern "C" int b2rl_replay_step(b2rl_replay *h, const b2rl_step_args *p, void *s
     h->step_seq++;
     const unsigned long long seq_base = (unsigned long long)h->step_seq << 32;
     // ---- sampler
-    a.s.sum = h->sum;
-    a.s.mn = h->mn;
-    a.s.st = h->st;
-    a.s.u = u_dev;
-    a.s.n = n;
-    a.s.levels = h->levels;
-    a.s.nslots = h->nslots;
-    a.s.T = h->levels + 1 < TOP_LEVELS ? h->levels + 1 : TOP_LEVELS;
-    a.s.D = h->levels - (a.s.T - 1);
-    a.s.slots_out = h->last_slots;
-    a.s.prio_out = h->last_prio;
-    a.s.index_out = (long long *)p->index_dev;
-    a.s.prio_user = p->priority_dev;
+    a.s = b2rl_sample_args(h, u_dev, n, p->index_dev, p->priority_dev);
     a.s.weight = p->weight_dev;
     a.s.prob = p->prob_dev;
     a.s.beta = p->beta;
     a.s.norm = p->norm;
     a.s.ready = h->ready_dev;
     a.s.seq_base = seq_base;
-    a.s.dbg_slow_every = b2rl_v6_slow_every();
-    a.s.dbg_eps_scale = b2rl_v6_eps_scale();
-    a.s.dbg_sleep_scale = b2rl_v6_sleep_scale();
     {
         static int want = -1; // B2RL_V6_CYCLES=1: clock64 sums per pipeline segment of the sampler
         if (want < 0) {

@@ -1,10 +1,11 @@
 // tree_dev.cuh -- device-side building blocks on the dense fp64 heaps, shared
 // by the stand-alone kernels (sampler.cu) and the fused replay step (step.cu):
 //
-//   exact_deep<D, FMA>()   bit-exact sequential sampler (main warp + two scout
+//   exact_deep<D>()        bit-exact sequential sampler (main warp + two scout
 //                          warps + a publisher warp)
+//   exact_deep_v6<D>()     bit-exact sampler deciding on approximate tables
 //   sample_parallel()      all descents concurrently on the frozen tree
-//   tree_update_paths()    priority write-back for <= 512 leaves: sorted
+//   tree_update_multi()    priority write-back for <= 512 leaves: sorted
 //                          paths, siblings prefetched in ONE round trip, the
 //                          level loop runs on shared memory only
 //
@@ -15,9 +16,12 @@
 #pragma once
 #include <math.h>
 
+#include <type_traits>
+
 #include "b2rl_internal.cuh"
 
 static constexpr int TOP_LEVELS = 14; // heap levels 0..13 -> 16383 nodes = 128 KB
+static constexpr int V6_T = 13;       // v6 keeps heap levels 0..12 in shared memory
 
 struct SampleArgs {
     double *sum;
@@ -47,9 +51,40 @@ struct SampleArgs {
     // path on every k-th draw / widen the decision margin; results must not change
     int dbg_slow_every;
     double dbg_eps_scale;
-    int dbg_sleep_scale; // env B2RL_V6_SLEEP: multiplies the helper warps' poll back-off
     long long *dbg_cycles; // optional [32]: clock64 sums per pipeline segment (tools/v6_cycles.py)
 };
+
+// The sampler that serves a draw of n from a tree with leaves at heap level `levels`; the
+// values double as the MODE of the fused k_replay_step<D, MODE> (step.cu).
+enum SamplerKind { SAMPLER_V5 = 0, SAMPLER_SMALL = 1, SAMPLER_PARALLEL = 2, SAMPLER_V6 = 3 };
+
+struct SamplerChoice {
+    SamplerKind kind;
+    int D; // template depth of exact_deep<D> / exact_deep_v6<D>; 0 for the others
+};
+
+// parallel mode -> sample_parallel; a tree that fits the TOP_LEVELS shared-memory levels
+// (SampleArgs::D == 0) -> exact_small; levels 17..21 with n <= 60000 -> v6 with D = levels - 12
+// (it stages 5..9 levels per draw, and its conflict table keeps draw ids in u16); every other
+// exact draw -> v5 with D = levels - 13.
+inline SamplerChoice choose_sampler(int mode, int levels, int n)
+{
+    if (mode == B2RL_SAMPLE_PARALLEL) return {SAMPLER_PARALLEL, 0};
+    if (levels < TOP_LEVELS) return {SAMPLER_SMALL, 0};
+    if (levels >= 17 && levels <= 21 && n <= 60000) return {SAMPLER_V6, levels - (V6_T - 1)};
+    return {SAMPLER_V5, levels - (TOP_LEVELS - 1)};
+}
+
+// f(std::integral_constant<int, d>{}) for a runtime d in [LO, HI]: turns the depth of a
+// SamplerChoice into the template argument of the kernel that serves it.
+template <int LO, int HI, typename F>
+cudaError_t with_depth(int d, F &&f)
+{
+    if constexpr (LO > HI)
+        return cudaErrorInvalidValue;
+    else
+        return d == LO ? f(std::integral_constant<int, LO>{}) : with_depth<LO + 1, HI>(d, f);
+}
 
 // ---------------------------------------------------------------------------
 // small PTX helpers
@@ -187,9 +222,9 @@ __device__ __forceinline__ float is_weight(double prob, double denom, double len
 // with a lane-constant multiplier: fma(-1, left, x) rounds x - left once,
 // exactly like __dsub_rn; fma(-0, left, x) = x + (-0) = x because tree values
 // are finite and >= 0.  The arithmetic of the winning lane is therefore bit
-// for bit the reference's (the bit-identity suite checks it).  FMA = false keeps the subtract + select form.
+// for bit the reference's (the bit-identity suite checks it).
 // ---------------------------------------------------------------------------
-template <int R, bool FMA>
+template <int R>
 __device__ __forceinline__ void spec_round(const double *val, int &node, double &pos, int lane)
 {
     static_assert(R >= 1 && R <= 5, "one round covers at most 5 levels");
@@ -207,11 +242,7 @@ __device__ __forceinline__ void spec_round(const double *val, int &node, double 
         const bool right = (li >> (R - 1 - j)) & 1;
         const bool lt = x < left[j];
         ok = ok && (lt != right);
-        if constexpr (FMA) {
-            x = __fma_rn(right ? -1.0 : -0.0, left[j], x);
-        } else {
-            if (right) x = __dsub_rn(x, left[j]);
-        }
+        x = __fma_rn(right ? -1.0 : -0.0, left[j], x);
     }
     unsigned m = __ballot_sync(0xffffffffu, ok);
     if constexpr (R < 5) m &= (1u << (1 << R)) - 1u;
@@ -220,13 +251,13 @@ __device__ __forceinline__ void spec_round(const double *val, int &node, double 
     node = (node << R) + win;
 }
 
-template <int L, bool FMA = true>
+template <int L>
 __device__ __forceinline__ void spec_descend(const double *val, int &node, double &pos, int lane)
 {
     if constexpr (L > 0) {
         constexpr int R = L >= 5 ? 5 : L;
-        spec_round<R, FMA>(val, node, pos, lane);
-        spec_descend<L - R, FMA>(val, node, pos, lane);
+        spec_round<R>(val, node, pos, lane);
+        spec_descend<L - R>(val, node, pos, lane);
     }
 }
 
@@ -264,7 +295,7 @@ __host__ __device__ constexpr size_t exact_deep_smem_bytes()
            sizeof(int) * (EX_RING + 16) + 16;
 }
 
-template <int D, bool FMA>
+template <int D>
 __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
 {
     constexpr int T = TOP_LEVELS;
@@ -321,7 +352,7 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
                 const double left = top[older];
                 if (!(pos < left)) { pos -= left; node = older ^ 1; }
             }
-            spec_descend<T - 2, FMA>(top, node, pos, lane);
+            spec_descend<T - 2>(top, node, pos, lane);
             double *dst = sub_pref + (k % NBUF) * SUBN;
             const unsigned unode = (unsigned)node;
             double2 tmp[NIT];
@@ -378,7 +409,7 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
                         node = older ^ 1;
                     }
                 }
-                spec_descend<T - 2, FMA>(top, node, pos, lane); // level 1 -> T-1
+                spec_descend<T - 2>(top, node, pos, lane); // level 1 -> T-1
                 const unsigned unode = (unsigned)node;
                 // ---- the D levels under `node`: staged by the scout, or fetched here
                 const double *sub;
@@ -410,7 +441,7 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
                     sub = sub_own;
                 }
                 int rel = 1;
-                spec_descend<D, FMA>(sub, rel, pos, lane);
+                spec_descend<D>(sub, rel, pos, lane);
                 const unsigned leafnode = (unode << D) + (unsigned)(rel - (1 << D));
                 const double prio = sub[rel];
                 // ---- _write(ix, 0.0): re-reduce the path, siblings first (:303)
@@ -705,22 +736,10 @@ __device__ __forceinline__ void sample_parallel(const SampleArgs &a, double *red
 }
 
 // ---------------------------------------------------------------------------
-// Priority write-back for up to UPD_MAX leaves (set_last_priority,
-// collections/prioritized.py:107-116, with priority_from_errors of
-// replay_buffers/prioritized.py:47-55 in front when TD errors are given).
-//
-// A level-synchronous walk over global memory costs one L2 round trip per
-// level (21 at 1 M capacity: 29 us for 512 leaves in round 1).  Here the
-// updated leaves are sorted, duplicates resolved (the reference writes in
-// order, so the LAST occurrence wins), and EVERY sibling any path can need is
-// fetched up front in one round trip; the level loop then runs on shared
-// memory only.  Sorted order makes the merge logic local: the paths below one
-// node form a contiguous run of entries, the first entry of a run is its
-// leader and carries the node's new value; two runs merge when they are the
-// two children of one parent.  Every parent is computed as fl(left + right) /
-// min(left, right) of its two children's final values, exactly what the
-// reference's bottom-up _write produces after the whole batch.
-// Called by all threads of the CTA.
+// Priority write-back (set_last_priority, collections/prioritized.py:107-116,
+// with priority_from_errors of replay_buffers/prioritized.py:47-55 in front
+// when TD errors are given): tree_update_multi below for up to UPD_MAX leaves,
+// the level-synchronous k_update (sampler.cu) for larger batches.
 // ---------------------------------------------------------------------------
 static constexpr int UPD_MAX = 512;
 
@@ -757,12 +776,6 @@ __device__ __forceinline__ void upd_stamp(const UpdateArgs &a, int slot)
     }
 }
 
-__host__ __device__ inline size_t update_paths_smem_bytes(int levels)
-{
-    // keys, leaf, runlen (int) + lead (int) + prio, vs, vm (double) + counts + siblings
-    return (size_t)UPD_MAX * (4 * 4 + 3 * 8) + 64 * 8 + (size_t)levels * UPD_MAX * 16;
-}
-
 __device__ __forceinline__ double priority_from_error(const UpdateArgs &a, int k)
 {
     // priority_from_errors, replay_buffers/prioritized.py:47-55
@@ -772,146 +785,57 @@ __device__ __forceinline__ double priority_from_error(const UpdateArgs &a, int k
     return (a.alpha == 0.5) ? sqrt(d) : pow(d, a.alpha);
 }
 
-__device__ __forceinline__ void tree_update_paths(const UpdateArgs &a, unsigned char *smem_raw)
+// The top `topl` <= 10 levels (<= 1023 nodes) recomputed from level `topl` in shared
+// memory (cheap barriers) instead of `topl` more global round trips: every node is a
+// pure function of its children, so recomputing all of them is exact.  Used by the
+// level-synchronous write-back (k_update) and append repair (k_tree_fix_small).
+// Called by all threads of the CTA.
+__device__ __forceinline__ void rebuild_top_levels(double *sum, double *mn, int topl)
 {
+    __shared__ double s_sum[2048], s_min[2048];
     const int tid = threadIdx.x, nt = blockDim.x;
-    const int lane = tid & 31, warp = tid >> 5, nw = nt >> 5;
-    double *prio_s = reinterpret_cast<double *>(smem_raw);      // [UPD_MAX] by draw index
-    double *vs = prio_s + UPD_MAX;                              // [UPD_MAX] by sorted entry
-    double *vm = vs + UPD_MAX;
-    double *red = vm + UPD_MAX;                                 // [64]
-    double *sib_s = red + 64;                                   // [levels][UPD_MAX]
-    double *sib_m = sib_s + (size_t)a.levels * UPD_MAX;
-    unsigned *keys = reinterpret_cast<unsigned *>(sib_m + (size_t)a.levels * UPD_MAX);
-    int *leaf = reinterpret_cast<int *>(keys + UPD_MAX);
-    int *runlen = leaf + UPD_MAX;
-    int *lead = runlen + UPD_MAX;
-    int *cnt = reinterpret_cast<int *>(red) + 64; // upper half of red[] as ints: [32..63] doubles
-
-    // ---- priorities, sort keys --------------------------------------------
-    double mx = 0.0;
-    for (int k = tid; k < UPD_MAX; k += nt) {
-        unsigned key = 0xffffffffu;
-        if (k < a.n) {
-            const double p = a.err ? priority_from_error(a, k) : a.new_prio[k];
-            if (a.err) a.new_prio[k] = p;
-            prio_s[k] = p;
-            mx = fmax(mx, p); // max_priority sees every value, :114
-            key = ((unsigned)a.slots[k] << 9) | (unsigned)k;
-        }
-        keys[k] = key;
+    const int base = 1 << topl;
+    for (int i = tid; i < base; i += nt) {
+        s_sum[base + i] = sum[base + i];
+        s_min[base + i] = mn[base + i];
     }
     __syncthreads();
-    // ---- bitonic sort of (slot, draw index) --------------------------------
-    for (int kk = 2; kk <= UPD_MAX; kk <<= 1) {
-        for (int j = kk >> 1; j > 0; j >>= 1) {
-            for (int i = tid; i < UPD_MAX; i += nt) {
-                const int ixj = i ^ j;
-                if (ixj > i) {
-                    const unsigned x = keys[i], y = keys[ixj];
-                    const bool up = (i & kk) == 0;
-                    if ((x > y) == up) {
-                        keys[i] = y;
-                        keys[ixj] = x;
-                    }
-                }
-            }
-            __syncthreads();
-        }
-    }
-    // ---- unique leaves (last occurrence of a slot wins), compaction ---------
-    // groups of 32 consecutive entries: ballot + popc, then a prefix over the
-    // <= 16 group counts
-    for (int g = warp; g < UPD_MAX / 32; g += nw) {
-        const int i = g * 32 + lane;
-        const bool w = i < a.n && (i == a.n - 1 || (keys[i + 1] >> 9) != (keys[i] >> 9));
-        const unsigned b = __ballot_sync(0xffffffffu, w);
-        if (lane == 0) cnt[g] = __popc(b);
-    }
-    __syncthreads();
-    int m = 0;
-    for (int g = 0; g < UPD_MAX / 32; g++) m += cnt[g];
-    for (int g = warp; g < UPD_MAX / 32; g += nw) {
-        const int i = g * 32 + lane;
-        const bool w = i < a.n && (i == a.n - 1 || (keys[i + 1] >> 9) != (keys[i] >> 9));
-        const unsigned b = __ballot_sync(0xffffffffu, w);
-        int base = 0;
-        for (int q = 0; q < g; q++) base += cnt[q];
-        if (w) {
-            const int pos = base + __popc(b & ((1u << lane) - 1u));
-            const int slot = (int)(keys[i] >> 9);
-            const double p = prio_s[keys[i] & 511u];
-            leaf[pos] = slot;
-            vs[pos] = p;
-            vm[pos] = p;
-            runlen[pos] = 1;
-            lead[pos] = 1;
-        }
-    }
-    __syncthreads();
-    // ---- leaves out, every sibling of every path in (one round trip) --------
-    for (int i = tid; i < m; i += nt) {
-        const long long ln = a.nslots + leaf[i];
-        a.sum[ln] = vs[i];
-        a.mn[ln] = vm[i];
-    }
-    for (int idx = tid; idx < m * a.levels; idx += nt) {
-        const int i = idx % m, s = idx / m; // s = sh - 1
-        const long long node = (a.nslots + leaf[i]) >> s;
-        sib_s[(size_t)s * UPD_MAX + i] = a.sum[node ^ 1];
-        sib_m[(size_t)s * UPD_MAX + i] = a.mn[node ^ 1];
-    }
-    __syncthreads();
-    // ---- level loop on shared memory ----------------------------------------
-    for (int s = 0; s < a.levels; s++) {
-        for (int i = tid; i < m; i += nt) {
-            if (!lead[i]) continue;
-            const long long node = (a.nslots + leaf[i]) >> s;
-            double ns, nm;
-            if ((node & 1) == 0) {
-                const int j = i + runlen[i];
-                if (j < m && ((a.nslots + leaf[j]) >> s) == node + 1) {
-                    ns = __dadd_rn(vs[i], vs[j]);
-                    nm = fmin(vm[i], vm[j]);
-                    runlen[i] += runlen[j];
-                } else {
-                    ns = __dadd_rn(vs[i], sib_s[(size_t)s * UPD_MAX + i]);
-                    nm = fmin(vm[i], sib_m[(size_t)s * UPD_MAX + i]);
-                }
-            } else {
-                if (i > 0 && ((a.nslots + leaf[i - 1]) >> s) == node - 1) {
-                    lead[i] = 0; // merged into the run on the left by its leader
-                    continue;
-                }
-                ns = __dadd_rn(sib_s[(size_t)s * UPD_MAX + i], vs[i]);
-                nm = fmin(sib_m[(size_t)s * UPD_MAX + i], vm[i]);
-            }
-            vs[i] = ns;
-            vm[i] = nm;
-            a.sum[node >> 1] = ns;
-            a.mn[node >> 1] = nm;
+    for (int lv = topl - 1; lv >= 0; lv--) {
+        const int w = 1 << lv;
+        for (int i = tid; i < w; i += nt) {
+            const int node = w + i;
+            s_sum[node] = s_sum[2 * node] + s_sum[2 * node + 1];
+            s_min[node] = fmin(s_min[2 * node], s_min[2 * node + 1]);
         }
         __syncthreads();
     }
-    // ---- max_priority, :114 ---------------------------------------------------
-    for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    if (lane == 0) red[warp] = mx;
-    __syncthreads();
-    if (tid == 0) {
-        for (int w = 1; w < nw; w++) mx = fmax(mx, red[w]);
-        if (mx > a.st->max_priority) a.st->max_priority = mx;
-        a.st->last_n = 0;
+    for (int i = 1 + tid; i < base; i += nt) {
+        sum[i] = s_sum[i];
+        mn[i] = s_min[i];
     }
-    __syncthreads();
 }
 
 // ---------------------------------------------------------------------------
-// Multi-CTA write-back.  tree_update_paths above is bound by ONE SM's L1TEX: the
-// ~21 x 512 x 2 scattered 8-byte sibling loads are ~20 k wavefronts, ~2 cycles
-// each (42 us measured).  The heap splits into 2^sl independent subtrees below
-// level sl (sl = min(7, levels)): CTA c runs the sorted-path algorithm on the
-// updated leaves that fall into subtree c (typically 4 of 512) -- all subtrees
-// in parallel on different SMs -- and the LAST CTA to arrive (atomic ticket)
+// Multi-CTA write-back of up to UPD_MAX leaves.
+//
+// A level-synchronous walk over global memory costs one L2 round trip per
+// level (21 at 1 M capacity: 29 us for 512 leaves in round 1).  The sorted-path
+// algorithm instead sorts the updated leaves, resolves duplicates (the
+// reference writes in order, so the LAST occurrence wins), and fetches EVERY
+// sibling any path can need up front in one round trip; the level loop then
+// runs on shared memory only.  Sorted order makes the merge logic local: the
+// paths below one node form a contiguous run of entries, the first entry of a
+// run is its leader and carries the node's new value; two runs merge when they
+// are the two children of one parent.  Every parent is computed as
+// fl(left + right) / min(left, right) of its two children's final values,
+// exactly what the reference's bottom-up _write produces after the whole batch.
+//
+// On one CTA that algorithm is bound by the SM's L1TEX: the ~21 x 512 x 2
+// scattered 8-byte sibling loads are ~20 k wavefronts, ~2 cycles each (42 us
+// measured).  So the heap splits into 2^sl independent subtrees below level sl
+// (sl = min(7, levels)): CTA c runs the sorted-path algorithm on the updated
+// leaves that fall into subtree c (typically 4 of 512) -- all subtrees in
+// parallel on different SMs -- and the LAST CTA to arrive (atomic ticket)
 // recomputes the 2^sl - 1 nodes above from the subtree roots (every node is a
 // pure function of its children, so recomputing untouched ones changes
 // nothing).  sync[0] = "write-back of launch `seq` complete" (release/acquire),
@@ -1052,7 +976,10 @@ __device__ __forceinline__ void tree_update_multi(const UpdateArgs &a, unsigned 
             }
             TEAM_SYNC();
             if (blockIdx.x == 0 && wt == 0) upd_stamp(a, 198);
-            // ---- level loop on shared memory (see tree_update_paths).  The node values go to
+            // ---- level loop on shared memory: at level s a leader whose node is a left child
+            // merges the run of its right sibling if that run exists, or else combines with the
+            // prefetched sibling; a right child whose left sibling leads a run was merged by that
+            // leader and stops leading.  The node values go to
             // global memory AFTER the loop, in one batch, so that no global store sits in front
             // of a level's barrier; the results are parked in the sibling slots (level s, entry i)
             // they were computed from, -1 marks the entries that wrote nothing at that level
@@ -1220,7 +1147,6 @@ __device__ __forceinline__ void tree_update_multi(const UpdateArgs &a, unsigned 
 // tools/v6_model.py is a CPU model of the decision logic (adversarial trees:
 // ties, 1e-30..1e+30 dynamic range, u on boundaries, mispredictions).
 // ===========================================================================
-static constexpr int V6_T = 13;
 static constexpr int V6_NSCOUT = 4;
 static constexpr int V6_LAG = 4;
 static constexpr int V6_NBUF = 6;
@@ -1285,7 +1211,7 @@ __device__ __forceinline__ void spec_round_margin(const double *val, int &node, 
     }
 }
 
-template <int D, bool FMA>
+template <int D>
 __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_d)
 {
     constexpr int T = V6_T;
@@ -1381,7 +1307,6 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
 
     const uint64_t pol = policy_evict_last();
     const double2 *sum2 = reinterpret_cast<const double2 *>(a.sum);
-    const unsigned slp = a.dbg_sleep_scale > 0 ? (unsigned)a.dbg_sleep_scale : 1u;
     const double root0 = etop[1];
     if (threadIdx.x == 0) s_misc[0] = root0;
     // decision margin (see the header comment / DESIGN.md)
@@ -1400,7 +1325,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             int m;
             while ((m = ld_acquire_smem(&flags[F_MAIN])) < k - LAG ||
                    ld_acquire_smem(&flags[F_ASCR]) < k - NBUF + 1)
-                __nanosleep(32 * slp);
+                __nanosleep(32);
             const long long tc1 = V6_CLK();
             // ---- prediction (any error only costs a slow draw): search the tables
             double pos = uk * (s_misc[0] - (double)(k - m) * pbar);
@@ -1591,7 +1516,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                             node = older ^ 1;
                         }
                     }
-                    spec_descend<T - 2, FMA>(etop, node, pos, lane); // level 1 -> 12
+                    spec_descend<T - 2>(etop, node, pos, lane); // level 1 -> 12
                     const unsigned unode = (unsigned)node;
 #pragma unroll
                     for (int it = 0; it < NIT; it++) {
@@ -1603,7 +1528,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                     }
                     __syncwarp();
                     rel = 1;
-                    spec_descend<D, FMA>(sub_own, rel, pos, lane);
+                    spec_descend<D>(sub_own, rel, pos, lane);
                     prio = sub_own[rel];
                     ord = (node - NTOP) ^ oflip;
                 } else {
@@ -1669,7 +1594,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
         long long c_await = 0, c_awork = 0;
         for (int k = 0; k < a.n; k++) {
             const long long ta0 = V6_CLK();
-            while (ld_acquire_smem(&flags[F_MAIN]) <= k) __nanosleep(20 * slp);
+            while (ld_acquire_smem(&flags[F_MAIN]) <= k) __nanosleep(20);
             const long long ta1 = V6_CLK();
             const int4 ev = *reinterpret_cast<const int4 *>(&ring[k % RING]);
             const unsigned lfn = (unsigned)a.nslots + (unsigned)ev.x; // heap index of the leaf
@@ -1726,7 +1651,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
         const double len = (double)(a.st->napp - npop);
         for (int k0 = 0; k0 < a.n; k0 += CHUNK) {
             const int kend = (a.n - k0 < CHUNK) ? a.n : k0 + CHUNK;
-            while (ld_acquire_smem(&flags[F_MAIN]) < kend) __nanosleep(200 * slp);
+            while (ld_acquire_smem(&flags[F_MAIN]) < kend) __nanosleep(200);
             if (k0 == 0) {
                 total = s_misc[1];
                 mroot = s_misc[2];

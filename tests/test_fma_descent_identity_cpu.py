@@ -1,5 +1,5 @@
-"""The arithmetic identity behind the opt-in DFMA descent of the exact sampler
-(csrc/sampler.cu, spec_round<R, FMA=true>): for finite x and finite left >= 0,
+"""The arithmetic identity behind the DFMA descent of the exact sampler
+(csrc/tree_dev.cuh, spec_round<R>): for finite x and finite left >= 0,
 
     fma(-1.0, left, x) == x - left      (one rounding, like __dsub_rn)
     fma(-0.0, left, x) == x             (bit for bit, including signed zeros)
