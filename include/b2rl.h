@@ -361,15 +361,18 @@ int b2rl_gae(const float *reward, const float *nonterminal, const float *v,
              float *v_teacher, double *scratch, float *stats, void *stream);
 
 /* PPO._lossfun (pfrl/agents/ppo.py:634-671) + the advantage standardisation
- * of :495 (adv_stats = {mean, std} or NULL).  clip_eps_vf < 0 selects the
- * unclipped value loss.  Outputs d loss/d{log_prob, entropy, v_pred} and
- * losses[4] = {total, policy, value, entropy}.  scratch: 3 doubles per 256
- * samples. */
+ * of :495 (adv_stats = {mean, std} or NULL).  The ratio is clamped to
+ * float(1 - clip_eps), float(1 + clip_eps), rounded once from double as torch
+ * rounds Python-float bounds.  clip_eps_vf < 0 selects the unclipped value
+ * loss.  Gradients follow torch's rules for the reference expression: min and
+ * max split a tie evenly, clamp passes the gradient on its bounds.  Outputs
+ * d loss/d{log_prob, entropy, v_pred} and losses[4] = {total, policy, value,
+ * entropy}.  scratch: 3 doubles per 256 samples. */
 int b2rl_ppo_loss(const float *log_prob, const float *entropy,
                   const float *v_pred, const float *log_prob_old,
                   const float *v_pred_old, const float *adv,
                   const float *v_teacher, const float *adv_stats, int32_t M,
-                  float clip_eps, float clip_eps_vf, float value_coef,
+                  double clip_eps, float clip_eps_vf, float value_coef,
                   float entropy_coef, float *g_log_prob, float *g_entropy,
                   float *g_v_pred, double *scratch, float *losses, void *stream);
 

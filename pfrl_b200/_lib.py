@@ -188,7 +188,7 @@ SIGNATURES = {
     "b2rl_quantile_huber_fwd": (_int, [_vp] * 4 + [_i32, _i32, _i32, _int] + [_vp] * 4),
     "b2rl_quantile_huber_bwd": (_int, [_vp] * 5 + [_i32, _i32, _i32, _int, _vp, _vp]),
     "b2rl_gae": (_int, [_vp] * 6 + [_i32, _i32, _dbl, _dbl] + [_vp] * 5),
-    "b2rl_ppo_loss": (_int, [_vp] * 8 + [_i32] + [ctypes.c_float] * 4 + [_vp] * 6),
+    "b2rl_ppo_loss": (_int, [_vp] * 8 + [_i32, _dbl] + [ctypes.c_float] * 3 + [_vp] * 6),
     "b2rl_polyak": (_int, [ctypes.POINTER(TensorPair), _i32, _dbl, _vp]),
     "b2rl_sac_target": (_int, [_vp] * 7 + [ctypes.c_float, _i32, _vp, _vp]),
     "b2rl_conv_nature1_fwd": (_int, [_vp, _vp, _vp, _i32, _vp, _vp]),

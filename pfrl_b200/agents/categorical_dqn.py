@@ -97,12 +97,10 @@ class CategoricalDQN(dqn.DQN):
         with torch.no_grad():
             next_p, z_values = self._next_distribution(exp_batch)
             self._last_q = qout.evaluate_actions(actions).detach()
-        v_min = float(z_values[0]) if not hasattr(self, "_z_cache") else self._z_cache[0]
-        if not hasattr(self, "_z_cache"):
-            self._z_cache = (float(z_values[0]), float(z_values[-1]), int(z_values.numel()))
-        v_min, v_max, _ = self._z_cache
+        # the model's own atoms, as the torch path uses them: a linspace rebuilt on the
+        # device differs from them in the last bit for some atoms
         loss, delta = fused.c51_loss(
             y, next_p, exp_batch["reward"], exp_batch["discount"],
-            exp_batch["is_state_terminal"], exp_batch.get("weights"), v_min, v_max,
-            mean=self.batch_accumulator == "mean")
+            exp_batch["is_state_terminal"], exp_batch.get("weights"),
+            mean=self.batch_accumulator == "mean", z=z_values)
         return loss, delta

@@ -116,7 +116,8 @@ struct PpoArgs {
     const float *log_prob_old, *v_pred_old, *adv, *v_teacher; // [M]
     const float *adv_stats; // [2] mean, std or null (no standardisation)
     int M;
-    float clip_eps, clip_eps_vf; // clip_eps_vf < 0: unclipped value loss
+    float ratio_lo, ratio_hi; // float32(1 -+ clip_eps), rounded once as torch.clamp does
+    float clip_eps_vf;        // < 0: unclipped value loss
     float value_coef, entropy_coef;
     float *g_log_prob, *g_entropy, *g_v_pred; // [M] d loss / d input
     double *partial;  // [gridDim.x, 3]
@@ -135,14 +136,15 @@ __global__ void __launch_bounds__(256) k_ppo_loss(PpoArgs a)
         if (a.adv_stats) adv = (adv - a.adv_stats[0]) / (a.adv_stats[1] + 1e-8f); // ppo.py:495
         const float ratio = expf(a.log_prob[i] - a.log_prob_old[i]);
         const float s1 = ratio * adv;
-        const float rc = fminf(fmaxf(ratio, 1.0f - a.clip_eps), 1.0f + a.clip_eps);
+        const float rc = fminf(fmaxf(ratio, a.ratio_lo), a.ratio_hi);
         const float s2 = rc * adv;
         lp = -(double)fminf(s1, s2);
-        // d(-min(s1, s2))/d log_prob: s1 active (or tie inside the clip range)
-        const bool inside = (ratio >= 1.0f - a.clip_eps) && (ratio <= 1.0f + a.clip_eps);
-        float g = 0.f;
-        if (s1 < s2 || (s1 == s2 && inside)) g = -adv * ratio;
-        a.g_log_prob[i] = g * invM;
+        // d(-min(s1, s2))/d log_prob by torch's rules: min splits a tie evenly and clamp
+        // passes the gradient on its bounds.  Inside [lo, hi] (bounds included) s2 == s1 and
+        // the two halves add up to all of it; outside, s2 is constant and a tie passes half.
+        const bool inside = ratio >= a.ratio_lo && ratio <= a.ratio_hi;
+        const float share = inside ? 1.0f : s1 < s2 ? 1.0f : s1 == s2 ? 0.5f : 0.0f;
+        a.g_log_prob[i] = -adv * ratio * share * invM;
 
         const float v = a.v_pred[i], vt = a.v_teacher[i];
         const float d = v - vt;
@@ -151,10 +153,15 @@ __global__ void __launch_bounds__(256) k_ppo_loss(PpoArgs a)
         if (a.clip_eps_vf >= 0.f) {
             const float vo = a.v_pred_old[i];
             const float lo = vo - a.clip_eps_vf, hi = vo + a.clip_eps_vf;
-            const float vc = fminf(fmaxf(v, lo), hi);
+            const float vlo = fmaxf(v, lo);
+            const float vc = fminf(vlo, hi);
             const float dc = vc - vt;
             const float lc = dc * dc;
-            const float pass = (v >= lo && v <= hi) ? 1.0f : 0.0f;
+            // _elementwise_clip is min(max(v, lo), hi) (ppo.py:28-33), not clamp: max and
+            // min each pass half the gradient at a tie, so v == lo or v == hi passes 0.5 and
+            // v == lo == hi (clip_eps_vf = 0) passes 0.25
+            const float pass = (v > lo ? 1.0f : v == lo ? 0.5f : 0.0f) *
+                               (vlo < hi ? 1.0f : vlo == hi ? 0.5f : 0.0f);
             if (lc > lvi) {
                 lvi = lc;
                 gv = 2.0f * dc * pass;
@@ -233,7 +240,7 @@ extern "C" int b2rl_gae(const float *reward, const float *nonterminal, const flo
 extern "C" int b2rl_ppo_loss(const float *log_prob, const float *entropy, const float *v_pred,
                              const float *log_prob_old, const float *v_pred_old,
                              const float *adv, const float *v_teacher, const float *adv_stats,
-                             int32_t M, float clip_eps, float clip_eps_vf, float value_coef,
+                             int32_t M, double clip_eps, float clip_eps_vf, float value_coef,
                              float entropy_coef, float *g_log_prob, float *g_entropy,
                              float *g_v_pred, double *scratch, float *losses, void *stream)
 {
@@ -243,9 +250,11 @@ extern "C" int b2rl_ppo_loss(const float *log_prob, const float *entropy, const 
     B2RL_REQUIRE(clip_eps_vf < 0.f || v_pred_old, B2RL_ERR_INVALID,
                  "ppo_loss: clipped value loss needs v_pred_old");
     B2RL_REQUIRE(M > 0, B2RL_ERR_RANGE, "ppo_loss: empty minibatch");
+    // torch.clamp(ratio, 1 - eps, 1 + eps) with Python floats: each bound is computed in
+    // double and rounded to fp32 once (1.0f - (float)eps differs for eps = 0.33, say)
     PpoArgs a{log_prob, entropy, v_pred, log_prob_old, v_pred_old, adv, v_teacher, adv_stats, M,
-              clip_eps, clip_eps_vf, value_coef, entropy_coef, g_log_prob, g_entropy, g_v_pred,
-              scratch, losses};
+              (float)(1.0 - clip_eps), (float)(1.0 + clip_eps), clip_eps_vf, value_coef,
+              entropy_coef, g_log_prob, g_entropy, g_v_pred, scratch, losses};
     a.ticket = b2rl_next_ticket();
     k_ppo_loss<<<(M + 255) / 256, 256, 0, (cudaStream_t)stream>>>(a);
     B2RL_CUDA(cudaGetLastError());

@@ -53,6 +53,8 @@ class _PpoLoss(torch.autograd.Function):
         g_v = torch.empty(M, dtype=torch.float32, device=dev)
         losses = torch.empty(4, dtype=torch.float32, device=dev)
         scratch = torch.empty(((M + 255) // 256) * 3, dtype=torch.float64, device=dev)
+        # clip_eps goes over as a double: the kernel rounds 1 -+ clip_eps to fp32 once, as
+        # torch.clamp does with the reference's Python-float bounds
         _lib.check(L.b2rl_ppo_loss(
             _p(_f32(log_prob).view(-1)), _p(_f32(entropy).view(-1)), _p(_f32(v_pred).view(-1)),
             _p(_f32(log_prob_old).view(-1)),
