@@ -333,6 +333,34 @@ int b2rl_td_loss_bwd(const float *y, const float *t, const float *weights,
                      int32_t n_actions, int clip_delta, int mean, float *grad_q,
                      void *stream);
 
+/* Targets of the advantage-learning and DPP agents (`mode`), fused with the
+ * scalar TD loss of b2rl_td_loss_fwd (same y/t/delta/loss outputs; the
+ * gradient is b2rl_td_loss_bwd's).  tq, tnq: target net at s and s' [B,nA];
+ * nq: online net at s' (DOUBLE_PAL only, else NULL).  T = r +
+ * discount*(1-terminal)*nextV; A(x) = x[a] - max x; L the DPP operator.
+ *   AL          nextV = max tnq            t = T + alpha*A(tq)
+ *   PAL         nextV = max tnq            t = T + alpha*max(A(tq), A(tnq))
+ *   DOUBLE_PAL  nextV = tnq[argmax nq]     t as PAL
+ *   DPP         L = sum softmax(eta*x)*x   t = tq[a] + T(nextV = L tnq) - L tq
+ *   DPPL        L = logsumexp(eta*x)/eta   t as DPP
+ *   DPP_GREEDY  L = max x                  t as DPP
+ * Replaces _compute_y_and_t of pfrl/agents/al.py, pal.py, double_pal.py and
+ * dpp.py.  alpha and eta are rounded to fp32 once (eta > 0 for DPP, DPPL). */
+#define B2RL_ADV_AL 0
+#define B2RL_ADV_PAL 1
+#define B2RL_ADV_DOUBLE_PAL 2
+#define B2RL_ADV_DPP 3
+#define B2RL_ADV_DPPL 4
+#define B2RL_ADV_DPP_GREEDY 5
+int b2rl_adv_td_loss_fwd(int mode, const float *q, const int64_t *action,
+                         const float *tq, const float *tnq, const float *nq,
+                         const float *reward, const float *discount,
+                         const float *terminal, const float *weights, int32_t B,
+                         int32_t n_actions, double alpha, double eta,
+                         int clip_delta, int mean, float *y_out, float *t_out,
+                         float *delta_out, float *scratch, float *loss_out,
+                         void *stream);
+
 /* Quantile Huber loss of IQN: |tau - 1[t<y]| * Huber(y, t) over [B, N, N'],
  * mean over N', sum over N (compute_eltwise_huber_quantile_loss and the value
  * losses of pfrl/agents/iqn.py:176-250); delta_out = mean over (N, N'). */

@@ -185,6 +185,8 @@ SIGNATURES = {
     "b2rl_c51_loss_bwd": (_int, [_vp] * 4 + [_i32, _i32, _int, _vp, _vp]),
     "b2rl_td_loss_fwd": (_int, [_vp] * 7 + [_i32, _i32, _int, _int] + [_vp] * 6),
     "b2rl_td_loss_bwd": (_int, [_vp] * 5 + [_i32, _i32, _int, _int, _vp, _vp]),
+    "b2rl_adv_td_loss_fwd": (_int, [_int] + [_vp] * 9 + [_i32, _i32, _dbl, _dbl, _int, _int]
+                             + [_vp] * 6),
     "b2rl_quantile_huber_fwd": (_int, [_vp] * 4 + [_i32, _i32, _i32, _int] + [_vp] * 4),
     "b2rl_quantile_huber_bwd": (_int, [_vp] * 5 + [_i32, _i32, _i32, _int, _vp, _vp]),
     "b2rl_gae": (_int, [_vp] * 6 + [_i32, _i32, _dbl, _dbl] + [_vp] * 5),

@@ -318,6 +318,10 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
                 mean=self.batch_accumulator == "mean")
             self._last_q = y.detach()
             return loss, delta
+        return self._compute_loss_torch(exp_batch, want_errors)
+
+    def _compute_loss_torch(self, exp_batch, want_errors=False):
+        """The reference's formulation: _compute_y_and_t, then the value loss."""
         y, t = self._compute_y_and_t(exp_batch)
         self._last_q = y.detach()
         delta = None

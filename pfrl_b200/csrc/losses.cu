@@ -2,6 +2,8 @@
 //
 // Replaces chains of small ATen launches + host round trips in the reference:
 //   pfrl/agents/dqn.py:44-104,388-470          Huber / MSE value loss, |y-t|
+//   pfrl/agents/al.py, pal.py, double_pal.py,  advantage-learning and DPP targets
+//     dpp.py (_compute_y_and_t)                (row max / argmax / softmax / logsumexp)
 //   pfrl/agents/categorical_dqn.py:7-57        _apply_categorical_projection
 //   pfrl/agents/categorical_dqn.py:60-97,178-204  cross entropy, per-sample
 //                                              priority error, weighted sum
@@ -148,27 +150,153 @@ struct TdArgs {
     unsigned ticket;
 };
 
+// r + discount * (1 - terminal) * next_v, dqn.py:405
+__device__ __forceinline__ float bellman_target(float r, float discount, float terminal,
+                                                float next_v)
+{
+    return __fadd_rn(r, __fmul_rn(__fmul_rn(discount, __fsub_rn(1.0f, terminal)), next_v));
+}
+
+// Writes y, t, |y - t| and the (weighted) Huber / 0.5 MSE term of sample i (dqn.py:44-104).
+__device__ __forceinline__ void td_outputs(float y, float t, int i, int clip_delta,
+                                           const float *weights, float *y_out, float *t_out,
+                                           float *delta_out, float *term)
+{
+    const float d = __fsub_rn(y, t);
+    const float ad = fabsf(d);
+    float l;
+    if (clip_delta)
+        l = ad < 1.0f ? __fmul_rn(__fmul_rn(0.5f, d), d) : __fsub_rn(ad, 0.5f);
+    else
+        l = __fmul_rn(__fmul_rn(d, d), 0.5f);
+    y_out[i] = y;
+    t_out[i] = t;
+    delta_out[i] = ad;
+    term[i] = weights ? __fmul_rn(l, weights[i]) : l;
+}
+
 __global__ void __launch_bounds__(256) k_td_fwd(TdArgs a)
 {
     __shared__ float sh[32];
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < a.B) {
         const float y = a.q[(size_t)i * a.nA + a.action[i]];
-        // r + discount * (1 - terminal) * next_q_max, dqn.py:405
-        const float t = __fadd_rn(
-            a.reward[i],
-            __fmul_rn(__fmul_rn(a.discount[i], __fsub_rn(1.0f, a.terminal[i])), a.next_q[i]));
-        const float d = __fsub_rn(y, t);
-        const float ad = fabsf(d);
-        float l;
-        if (a.clip_delta)
-            l = ad < 1.0f ? __fmul_rn(__fmul_rn(0.5f, d), d) : __fsub_rn(ad, 0.5f);
-        else
-            l = __fmul_rn(__fmul_rn(d, d), 0.5f);
-        a.y_out[i] = y;
-        a.t_out[i] = t;
-        a.delta_out[i] = ad;
-        a.term[i] = a.weights ? __fmul_rn(l, a.weights[i]) : l;
+        const float t = bellman_target(a.reward[i], a.discount[i], a.terminal[i], a.next_q[i]);
+        td_outputs(y, t, i, a.clip_delta, a.weights, a.y_out, a.t_out, a.delta_out, a.term);
+    }
+    finish_sum(a.term, a.B, a.mean ? (float)a.B : 1.0f, a.loss_out, sh, a.ticket);
+}
+
+// ---------------------------------------------------------------------------
+// Advantage-learning and DPP targets (AL, PAL, DoublePAL, DPP, DPPL, DPPGreedy):
+// y = Q(s)[a] as for DQN, t from row reductions over the target net's action
+// values at s and s'.  One warp per sample, lanes strided over the actions.
+// ---------------------------------------------------------------------------
+constexpr int ADV_WARPS = 8;
+
+struct AdvTdArgs {
+    const float *q;          // [B, nA] online net at s
+    const long long *action; // [B]
+    const float *tq, *tnq;   // [B, nA] target net at s and s'
+    const float *nq;         // [B, nA] online net at s' (DOUBLE_PAL) or null
+    const float *reward, *discount, *terminal, *weights;
+    float alpha;             // fp32(alpha), as torch rounds a Python float factor
+    float eta, inv_eta;      // fp32(eta) and fp32(1 / fp32(eta)): torch's x / eta on CUDA
+    int mode, B, nA, clip_delta, mean;
+    float *y_out, *t_out, *delta_out, *term, *loss_out;
+    unsigned ticket;
+};
+
+// v at j beats the best so far (bv at bj): torch's max / argmax order, NaN
+// greatest, the first index among equals.
+__device__ __forceinline__ bool beats(float v, int j, float bv, int bj)
+{
+    if (isnan(v)) return !isnan(bv) || j < bj;
+    if (isnan(bv)) return false;
+    return v > bv || (v == bv && j < bj);
+}
+
+// max over row[0..n) and its first index, on every lane of the warp (n >= 1)
+__device__ __forceinline__ float warp_row_max(const float *row, int n, int lane, int *idx)
+{
+    float bv = 0.f;
+    int bj = -1; // this lane has seen no element yet
+    for (int j = lane; j < n; j += 32) {
+        const float v = row[j];
+        if (bj < 0 || beats(v, j, bv, bj)) bv = v, bj = j;
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        const float v = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int j = __shfl_xor_sync(0xffffffffu, bj, o);
+        if (j >= 0 && (bj < 0 || beats(v, j, bv, bj))) bv = v, bj = j;
+    }
+    *idx = bj;
+    return bv;
+}
+
+// DPP's L operators over one row of action values x with maximum xmax, on every lane.
+// Softmax and logsumexp take z = fp32(eta) * x first, as `eta * q_values` does, and
+// subtract max z before exp (torch's softmax and logsumexp do the same).
+__device__ __forceinline__ float warp_l_operator(int mode, const float *row, int n, int lane,
+                                                 float xmax, float eta, float inv_eta)
+{
+    if (mode == B2RL_ADV_DPP_GREEDY) return xmax;
+    // eta > 0, so max z = fp32(eta * max x)
+    float zmax = __fmul_rn(eta, xmax);
+    if (mode == B2RL_ADV_DPPL && isinf(zmax)) zmax = 0.f; // logsumexp's masked_fill
+    float s = 0.f, sx = 0.f;
+    for (int j = lane; j < n; j += 32) {
+        const float x = row[j];
+        const float e = expf(__fsub_rn(__fmul_rn(eta, x), zmax));
+        s = __fadd_rn(s, e);
+        sx = __fadd_rn(sx, __fmul_rn(e, x));
+    }
+    s = warp_sum(s);
+    if (mode == B2RL_ADV_DPPL) // logsumexp(eta * x) / eta, dpp.py:105
+        return __fmul_rn(__fadd_rn(logf(s), zmax), inv_eta);
+    // sum(softmax(eta * x) * x), action_value.py:78-79: normalise once after the sum
+    sx = warp_sum(sx);
+    return __fdiv_rn(sx, s);
+}
+
+__global__ void __launch_bounds__(ADV_WARPS * 32) k_adv_td_fwd(AdvTdArgs a)
+{
+    __shared__ float sh[32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * ADV_WARPS + warp;
+    if (i < a.B) {
+        const int n = a.nA;
+        const size_t off = (size_t)i * n;
+        const int act = (int)a.action[i];
+        const float *tq = a.tq + off, *tnq = a.tnq + off;
+        int jmax;
+        const float tq_max = warp_row_max(tq, n, lane, &jmax);
+        const float tnq_max = warp_row_max(tnq, n, lane, &jmax);
+        const float tq_a = tq[act], tnq_a = tnq[act];
+        const float r = a.reward[i], disc = a.discount[i], term = a.terminal[i];
+        float t;
+        if (a.mode == B2RL_ADV_AL || a.mode == B2RL_ADV_PAL || a.mode == B2RL_ADV_DOUBLE_PAL) {
+            float next_v = tnq_max;
+            if (a.mode == B2RL_ADV_DOUBLE_PAL) { // Q'(s', argmax_a Q(s', a)), double_pal.py:48-51
+                int jg;
+                warp_row_max(a.nq + off, n, lane, &jg);
+                next_v = tnq[jg];
+            }
+            const float tb = bellman_target(r, disc, term, next_v);
+            float adv = __fsub_rn(tq_a, tq_max); // target_qout.compute_advantage, al.py:69
+            if (a.mode != B2RL_ADV_AL) {         // torch.max(cur, next), pal.py:73-77
+                const float adv_next = __fsub_rn(tnq_a, tnq_max);
+                adv = (isnan(adv) || adv > adv_next) ? adv : adv_next;
+            }
+            t = __fadd_rn(tb, __fmul_rn(a.alpha, adv));
+        } else { // Q'(s,a) + (r + disc (1 - term) L Q'(s')) - L Q'(s), dpp.py:34-76
+            const float l_next = warp_l_operator(a.mode, tnq, n, lane, tnq_max, a.eta, a.inv_eta);
+            const float l_cur = warp_l_operator(a.mode, tq, n, lane, tq_max, a.eta, a.inv_eta);
+            t = __fsub_rn(__fadd_rn(tq_a, bellman_target(r, disc, term, l_next)), l_cur);
+        }
+        if (lane == 0)
+            td_outputs(a.q[off + act], t, i, a.clip_delta, a.weights, a.y_out, a.t_out,
+                       a.delta_out, a.term);
     }
     finish_sum(a.term, a.B, a.mean ? (float)a.B : 1.0f, a.loss_out, sh, a.ticket);
 }
@@ -317,6 +445,45 @@ extern "C" int b2rl_td_loss_fwd(const float *q, const int64_t *action, const flo
              n_actions, clip_delta, mean, y_out, t_out, delta_out, scratch, loss_out};
     a.ticket = b2rl_next_ticket();
     k_td_fwd<<<(B + 255) / 256, 256, 0, (cudaStream_t)stream>>>(a);
+    B2RL_CUDA(cudaGetLastError());
+    return B2RL_OK;
+}
+
+extern "C" int b2rl_adv_td_loss_fwd(int mode, const float *q, const int64_t *action,
+                                    const float *tq, const float *tnq, const float *nq,
+                                    const float *reward, const float *discount,
+                                    const float *terminal, const float *weights, int32_t B,
+                                    int32_t n_actions, double alpha, double eta, int clip_delta,
+                                    int mean, float *y_out, float *t_out, float *delta_out,
+                                    float *scratch, float *loss_out, void *stream)
+{
+    B2RL_REQUIRE(q && action && tq && tnq && reward && discount && terminal && y_out && t_out &&
+                     delta_out && scratch && loss_out, B2RL_ERR_INVALID,
+                 "adv_td_loss_fwd: null argument");
+    B2RL_REQUIRE(mode >= B2RL_ADV_AL && mode <= B2RL_ADV_DPP_GREEDY, B2RL_ERR_INVALID,
+                 "adv_td_loss_fwd: unknown mode %d", mode);
+    B2RL_REQUIRE(mode != B2RL_ADV_DOUBLE_PAL || nq, B2RL_ERR_INVALID,
+                 "adv_td_loss_fwd: DOUBLE_PAL needs the online net's next-state values");
+    B2RL_REQUIRE(B > 0 && n_actions > 0, B2RL_ERR_RANGE, "adv_td_loss_fwd: empty batch");
+    const bool softmax_mode = mode == B2RL_ADV_DPP || mode == B2RL_ADV_DPPL;
+    B2RL_REQUIRE(!softmax_mode || (float)eta > 0.f, B2RL_ERR_RANGE,
+                 "adv_td_loss_fwd: need eta > 0, got %g", eta);
+    AdvTdArgs a{q, (const long long *)action, tq, tnq, nq, reward, discount, terminal, weights};
+    a.alpha = (float)alpha;
+    a.eta = (float)eta;
+    a.inv_eta = softmax_mode ? 1.0f / a.eta : 0.f;
+    a.mode = mode;
+    a.B = B;
+    a.nA = n_actions;
+    a.clip_delta = clip_delta;
+    a.mean = mean;
+    a.y_out = y_out;
+    a.t_out = t_out;
+    a.delta_out = delta_out;
+    a.term = scratch;
+    a.loss_out = loss_out;
+    a.ticket = b2rl_next_ticket();
+    k_adv_td_fwd<<<(B + ADV_WARPS - 1) / ADV_WARPS, ADV_WARPS * 32, 0, (cudaStream_t)stream>>>(a);
     B2RL_CUDA(cudaGetLastError());
     return B2RL_OK;
 }

@@ -107,6 +107,54 @@ def td_loss(q, action, next_q, reward, discount, terminal, weights, clip_delta=T
     return _TdLoss.apply(q, action, next_q, reward, discount, terminal, weights, clip_delta, mean)
 
 
+ADV_MODES = {"al": 0, "pal": 1, "double_pal": 2, "dpp": 3, "dppl": 4, "dpp_greedy": 5}
+
+
+class _AdvTdLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, action, target_q, target_next_q, next_q, reward, discount, terminal,
+                weights, mode, alpha, eta, clip_delta, mean):
+        L = _lib.load()
+        B, nA = q.shape
+        qc = _f32(q)
+        act = action.detach().long().contiguous()
+        w = None if weights is None else _f32(weights)
+        nq = None if next_q is None else _f32(next_q)
+        dev = q.device
+        y = torch.empty(B, dtype=torch.float32, device=dev)
+        t = torch.empty(B, dtype=torch.float32, device=dev)
+        delta = torch.empty(B, dtype=torch.float32, device=dev)
+        scratch = torch.empty(B, dtype=torch.float32, device=dev)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        _lib.check(L.b2rl_adv_td_loss_fwd(
+            ADV_MODES[mode], _p(qc), _p(act), _p(_f32(target_q)), _p(_f32(target_next_q)), _p(nq),
+            _p(_f32(reward)), _p(_f32(discount)), _p(_f32(terminal)), _p(w), B, nA, float(alpha),
+            float(eta), int(clip_delta), int(mean), _p(y), _p(t), _p(delta), _p(scratch), _p(loss),
+            _stream()))
+        ctx.save_for_backward(y, t, act, w if w is not None else torch.empty(0, device=dev))
+        ctx.has_w = w is not None
+        ctx.cfg = (B, nA, int(clip_delta), int(mean))
+        ctx.mark_non_differentiable(delta, y, t)
+        return loss, delta, y, t
+
+    @staticmethod
+    def backward(ctx, g_loss, *unused):
+        # the target carries no gradient: d loss / d q is the scalar TD loss's
+        return (_TdLoss.backward(ctx, g_loss)[0],) + (None,) * 13
+
+
+def adv_td_loss(q, action, target_q, target_next_q, reward, discount, terminal, weights, mode,
+                alpha=0.9, eta=1.0, next_q=None, clip_delta=True, mean=True):
+    """TD loss with the target of an advantage-learning or DPP agent.
+
+    ``mode`` is one of ``ADV_MODES``: "al", "pal", "double_pal" (needs ``next_q``, the online
+    net at s'), "dpp", "dppl", "dpp_greedy".  ``target_q`` / ``target_next_q`` are the target
+    net's action values at s and s'.  Only ``q`` (the online net at s) gets a gradient.
+    Returns (loss, |y - t|, y, t)."""
+    return _AdvTdLoss.apply(q, action, target_q, target_next_q, next_q, reward, discount,
+                            terminal, weights, mode, alpha, eta, clip_delta, mean)
+
+
 class _QuantileHuber(torch.autograd.Function):
     @staticmethod
     def forward(ctx, y, t, taus, weights, mean):

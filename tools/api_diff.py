@@ -18,6 +18,7 @@ from oracle.refimport import import_reference  # noqa: E402
 
 CALLABLES = """
 agents.DQN agents.DoubleDQN agents.CategoricalDQN agents.CategoricalDoubleDQN agents.IQN
+agents.AL agents.PAL agents.DoublePAL agents.DPP agents.dpp.DPPL agents.dpp.DPPGreedy
 agents.PPO agents.A2C agents.SoftActorCritic agents.TD3 agents.DDPG
 replay_buffers.ReplayBuffer replay_buffers.PrioritizedReplayBuffer
 replay_buffer.batch_experiences replay_buffer.ReplayUpdater utils.batch_states
@@ -43,6 +44,7 @@ action_value.SingleActionValue
 
 METHOD_CLASSES = """
 agents.DQN agents.CategoricalDoubleDQN agents.IQN agents.PPO agents.A2C agents.SoftActorCritic
+agents.AL agents.PAL agents.DoublePAL agents.DPP agents.dpp.DPPL agents.dpp.DPPGreedy
 agents.TD3 agents.DDPG replay_buffers.ReplayBuffer replay_buffers.PrioritizedReplayBuffer
 replay_buffer.ReplayUpdater nn.EmpiricalNormalization nn.FactorizedNoisyLinear
 envs.MultiprocessVectorEnv envs.SerialVectorEnv wrappers.VectorFrameStack

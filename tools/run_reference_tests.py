@@ -41,6 +41,8 @@ DEFAULT = [
     "agents_tests/test_iqn.py", "agents_tests/test_ppo.py", "agents_tests/test_a2c.py",
     "agents_tests/test_soft_actor_critic.py", "agents_tests/test_td3.py",
     "agents_tests/test_ddpg.py",
+    "agents_tests/test_al.py", "agents_tests/test_pal.py", "agents_tests/test_double_pal.py",
+    "agents_tests/test_dpp.py",
 ]
 
 PLUGIN = '''
