@@ -500,7 +500,7 @@ typedef struct b2rl_gemm_output {
     int32_t ld;              /* dense: C[m * ld + n] */
     const int32_t *row_tab;  /* scatter when not NULL */
     int32_t col_stride;
-    const float *bias;       /* [N] or NULL */
+    const float *bias;       /* [N] or NULL; 4-byte aligned, may start at any float */
     int32_t relu;
 } b2rl_gemm_output;
 /* Debug aid: %globaltimer stamps of the phases of every CTA of the following launches are

@@ -88,6 +88,7 @@ struct Operand {
 struct GemmArgs {
     Operand A, B;
     const float *bias;
+    int bias_vec;        // bias is 16-byte aligned: the dense epilogue may read it as float4
     float *C;            // final output (splits == 1) ...
     float *partial;      // ... or [splits][M][N] partial sums
     const int *c_row_tab; // scatter: C[m, n] at c_row_tab[m] + n * c_col_stride
@@ -182,8 +183,11 @@ template <> struct Wgmma<64> {
 
 // x = hi + lo (+ <= 2^-22 |x|), both exactly representable in TF32 (10-bit mantissa, low 13
 // bits zero); rounding to nearest in integer arithmetic on the sign-magnitude bit pattern
-// (plain integer instructions instead of the conversion pipe).  x - hi is exact.  Non-finite
-// inputs come out as NaN.
+// (plain integer instructions instead of the conversion pipe).  x - hi is exact.  Inf and
+// most NaNs give non-finite results (Inf gives hi = Inf and, through x - hi, a zero lo).  A NaN
+// whose leading mantissa bits are all set (0x7fffffff, the NaN CUDA's arithmetic produces) does
+// not: the rounding carry runs into the sign bit and leaves hi = lo = -0, so it drops out of
+// the product.  Testing every element for it costs 5-7% of the product time on an H100.
 __device__ __forceinline__ void split_tf32(float x, uint32_t &hi, uint32_t &lo)
 {
     hi = (__float_as_uint(x) + 0x1000u) & 0xffffe000u;
@@ -498,7 +502,11 @@ __global__ void __launch_bounds__(THREADS, 1) k_gemm_tf32x3(const __grid_constan
             float *o = out + (size_t)(m0 + rr) * ldo + n0 + cc;
             if (n0 + cc + 4 <= g.N) {
                 if (bias_relu && g.bias) {
-                    const float4 bv = __ldg(reinterpret_cast<const float4 *>(g.bias + n0 + cc));
+                    const float *bp = g.bias + n0 + cc;
+                    const float4 bv = g.bias_vec
+                                          ? __ldg(reinterpret_cast<const float4 *>(bp))
+                                          : make_float4(__ldg(bp), __ldg(bp + 1), __ldg(bp + 2),
+                                                        __ldg(bp + 3));
                     x.x += bv.x, x.y += bv.y, x.z += bv.z, x.w += bv.w;
                 }
                 if (bias_relu && g.relu)
@@ -689,12 +697,13 @@ extern "C" int b2rl_gemm_tf32x3_ex(const b2rl_gemm_operand *A, const b2rl_gemm_o
     if (rc != B2RL_OK) return rc;
     rc = fill_operand(B, N, K, &g.B, "B");
     if (rc != B2RL_OK) return rc;
-    g.bias = C->bias, g.C = C->data;
+    // a bias that is a view into a larger buffer (a flat parameter vector) may start at any float
+    g.bias = C->bias, g.bias_vec = ((uintptr_t)C->bias & 15) == 0, g.C = C->data;
     g.c_row_tab = C->row_tab, g.c_col_stride = C->col_stride;
     B2RL_REQUIRE(C->row_tab || C->ld >= N, B2RL_ERR_RANGE,
                  "gemm_tf32x3: leading dimension of C smaller than its rows");
-    B2RL_REQUIRE(((uintptr_t)C->data & 3) == 0, B2RL_ERR_INVALID,
-                 "gemm_tf32x3: C must be 4-byte aligned");
+    B2RL_REQUIRE(((uintptr_t)C->data & 3) == 0 && ((uintptr_t)C->bias & 3) == 0,
+                 B2RL_ERR_INVALID, "gemm_tf32x3: C and bias must be 4-byte aligned");
     g.M = M, g.N = N, g.K = K, g.ldc = C->ld;
     g.c_vec = (!C->row_tab && ((uintptr_t)C->data & 15) == 0 && C->ld % 4 == 0);
     g.relu = C->relu ? 1 : 0;

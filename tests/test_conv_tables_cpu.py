@@ -48,7 +48,8 @@ def _scatter(C, prod, out):
     (3, 4, 20, 20, 6, 4, 4, 2),    # conv2-like
     (2, 5, 9, 9, 7, 3, 3, 1),      # conv3-like
     (2, 4, 28, 28, 5, 8, 8, 4),    # conv1-like (16 stride phases)
-    (2, 3, 11, 13, 5, 3, 3, 2),    # remainder rows / columns that no window covers
+    (2, 3, 11, 13, 5, 3, 3, 2),    # odd sizes whose windows still cover every pixel
+    (2, 3, 12, 14, 5, 3, 3, 2),    # remainder rows / columns that no window covers
     (2, 2, 9, 9, 3, 2, 2, 3),      # stride > kernel: some input pixels get no gradient
 ])
 def test_tables_describe_conv_forward_dgrad_wgrad(B, IC, H, W, OC, KH, KW, s):

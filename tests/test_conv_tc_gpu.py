@@ -18,7 +18,9 @@ LAYERS = [
     (32, 64, 9, 9, 64, 3, 1),
     (512, 64, 9, 9, 64, 3, 1),
     (32, 4, 84, 84, 32, 8, 4),
-    (9, 3, 11, 13, 5, 3, 2),      # ragged: odd sizes, stride 2 with a remainder
+    (9, 3, 11, 13, 5, 3, 2),      # ragged: odd sizes, stride 2, windows cover every pixel
+    (9, 3, 12, 14, 5, 3, 2),      # stride 2 with a remainder: the last row and column unread
+    (8, 2, 9, 9, 3, 2, 3),        # stride > kernel: input gradient pixels zero-filled
     (8, 2, 7, 7, 3, 2, 1),
 ]
 

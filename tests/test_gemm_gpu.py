@@ -1,9 +1,12 @@
 """K10: the wgmma 3xTF32 product (csrc/gemm.cu, b2rl_gemm_tf32x3) against an fp64 product.
 
-Tolerance (written here, as the task asks): every element within 2^-18 * (|A| . |B|^T) of the
-fp64 result -- the worst case of the split (two operands at 2^-22 each plus the dropped lo.lo
-term, with margin); in practice the error sits next to cuBLAS' own fp32 SGEMM error, which the
-test prints and bounds too (<= 4x cuBLAS' max error + 1e-6).  The shapes are the Rainbow / DQN
+Tolerance: on these random-sign operands every element within 2^-18 * (|A| . |B|^T) of the
+fp64 result.  This is what random signs give, not a worst case: the tensor core truncates on
+every accumulation, so on same-sign data the error grows with the number of k steps per split
+(2^-14 at K = 8192 in one split).  tests/test_tensor_core_fp64_gpu.py derives the K-dependent
+bound that holds for any data and checks every path against it.  The error also sits next to
+cuBLAS' own fp32 SGEMM error, which the test prints and bounds too (<= 4x cuBLAS' max error
++ 1e-6).  The shapes are the Rainbow / DQN
 layers at B = 512 (pfrl/q_functions/dueling_dqn.py:67-129) in all three orientations (forward,
 dX, dW), ragged edges, unaligned leading dimensions, strided (chunked) inputs.
 """
