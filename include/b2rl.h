@@ -225,6 +225,57 @@ int b2rl_replay_gather(b2rl_replay *h, const int64_t *index_dev, int32_t n,
                        void *stream);
 
 /* ------------------------------------------------------------------------
+ * Sequence gather for recurrent (episodic) updates; replaces
+ * batch_recurrent_experiences (pfrl/replay_buffer.py:219-287) + the per-episode
+ * batch_states + pack_sequence (pfrl/utils/recurrent.py:249-277) + the H2D copy.
+ * Store built with n_step = 1.  Sequence b is the records first[b] ..
+ * first[b] + len[b] - 1 (logical indices); its step t is written at the
+ * packed row  sum_{t' < t} batch_sizes[t'] + b  (pack_sequence order, time
+ * major), batch_sizes[t'] = #{b : len[b] > t'}.
+ * ---------------------------------------------------------------------- */
+#define B2RL_SEQ_MAX_B 1024
+#define B2RL_SEQ_MAX_LEAVES 8
+
+typedef struct {
+    void *state;      /* [N][stack*part_bytes] bytes, or f32 (U8_TO_F32), N = sum(len) */
+    void *next_state; /* same layout                                          */
+    void *action;     /* [N][action_bytes]                                    */
+    float *reward;    /* [N] fp32 rounding of the stored fp64 reward          */
+    float *terminal;  /* [N] 1.0 / 0.0                                        */
+} b2rl_seq_out;
+
+/* Recurrent states of the records, kept by the caller in HBM: row r of
+ * `ring` holds the state (r, 0) and the next state (r, 1) of the record whose
+ * absolute append index a satisfies a % ring_rows == r, flattened to
+ * row_floats floats each; present[r][k] = 0 marks a stored None.  The state
+ * of each sequence's FIRST record is written to the leaves: leaf i takes the
+ * floats [offset[i], offset[i] + d0[i] * inner[i]) of the row as a
+ * [d0, inner] block and writes it as out[i] = f32 [d0][B][inner] (zeros for
+ * None), i.e. concatenate_recurrent_states of [d0, inner]-shaped entries. */
+typedef struct {
+    const float *ring;       /* [ring_rows][2][row_floats] */
+    const uint8_t *present;  /* [ring_rows][2] */
+    int64_t ring_rows;
+    int32_t row_floats;
+    int32_t n_leaves;
+    int32_t offset[B2RL_SEQ_MAX_LEAVES], d0[B2RL_SEQ_MAX_LEAVES], inner[B2RL_SEQ_MAX_LEAVES];
+    float *out_state[B2RL_SEQ_MAX_LEAVES];
+    float *out_next_state[B2RL_SEQ_MAX_LEAVES];
+} b2rl_seq_states;
+
+/* first_host / len_host / end_host: B host arrays, 1 <= B <= B2RL_SEQ_MAX_B;
+ * end[b] is one past the last record of the episode sequence b is cut from.
+ * Requires 0 <= first[b], len[b] >= 1, first[b] + len[b] <= end[b] <= live
+ * records, len non-increasing (a stable sort by length, longest first), else
+ * B2RL_ERR_RANGE.  states may be NULL.  One launch, no synchronisation, no
+ * allocation. */
+int b2rl_replay_gather_sequences(b2rl_replay *h, const int64_t *first_host,
+                                 const int32_t *len_host, const int64_t *end_host,
+                                 int32_t B, int obs_mode, float obs_scale,
+                                 const b2rl_seq_out *out, const b2rl_seq_states *states,
+                                 void *stream);
+
+/* ------------------------------------------------------------------------
  * Fused replay step: ONE persistent launch per minibatch that
  *   1. writes back the priorities of the PREVIOUS sample if its TD errors were
  *      registered with b2rl_per_defer_errors (set_last_priority,

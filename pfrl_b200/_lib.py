@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 LIB_PATH = os.path.join(CSRC, "libb2rl.so")
-SOURCES = ["replay.cu", "sampler.cu", "step.cu", "gather.cu", "losses.cu", "ppo.cu", "sac.cu", "conv.cu", "gemm.cu"]
+SOURCES = ["replay.cu", "sampler.cu", "step.cu", "gather.cu", "episodic.cu", "losses.cu", "ppo.cu", "sac.cu", "conv.cu", "gemm.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
@@ -113,6 +113,27 @@ class StepArgs(ctypes.Structure):
     ]
 
 
+SEQ_MAX_B, SEQ_MAX_LEAVES = 1024, 8
+
+
+class SeqOut(ctypes.Structure):
+    """b2rl_seq_out (include/b2rl.h)."""
+    _fields_ = [("state", ctypes.c_void_p), ("next_state", ctypes.c_void_p),
+                ("action", ctypes.c_void_p), ("reward", ctypes.c_void_p),
+                ("terminal", ctypes.c_void_p)]
+
+
+class SeqStates(ctypes.Structure):
+    """b2rl_seq_states (include/b2rl.h)."""
+    _fields_ = [("ring", ctypes.c_void_p), ("present", ctypes.c_void_p),
+                ("ring_rows", ctypes.c_int64), ("row_floats", ctypes.c_int32),
+                ("n_leaves", ctypes.c_int32),
+                ("offset", ctypes.c_int32 * SEQ_MAX_LEAVES), ("d0", ctypes.c_int32 * SEQ_MAX_LEAVES),
+                ("inner", ctypes.c_int32 * SEQ_MAX_LEAVES),
+                ("out_state", ctypes.c_void_p * SEQ_MAX_LEAVES),
+                ("out_next_state", ctypes.c_void_p * SEQ_MAX_LEAVES)]
+
+
 class GemmOperand(ctypes.Structure):
     """b2rl_gemm_operand (include/b2rl.h)."""
     _fields_ = [("data", ctypes.c_void_p), ("mode", ctypes.c_int32), ("ld", ctypes.c_int32),
@@ -181,6 +202,9 @@ SIGNATURES = {
     "b2rl_per_flush": (_int, [_vp, _vp]),
     "b2rl_replay_gather": (
         _int, [_vp, _vp, _i32, _vp, _int, ctypes.c_float, ctypes.POINTER(BatchOut), _vp]),
+    "b2rl_replay_gather_sequences": (
+        _int, [_vp, _vp, _vp, _vp, _i32, _int, ctypes.c_float, ctypes.POINTER(SeqOut),
+               ctypes.POINTER(SeqStates), _vp]),
     "b2rl_c51_loss_fwd": (_int, [_vp] * 7 + [_i32, _i32, _int] + [_vp] * 5),
     "b2rl_c51_loss_bwd": (_int, [_vp] * 4 + [_i32, _i32, _int, _vp, _vp]),
     "b2rl_td_loss_fwd": (_int, [_vp] * 7 + [_i32, _i32, _int, _int] + [_vp] * 6),

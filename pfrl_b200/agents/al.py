@@ -13,6 +13,8 @@ class AL(dqn.DQN):
     (default 0.9); everything else is DQN's.
     """
 
+    _recurrent_supported = False
+
     _fused_mode = "al"
 
     def __init__(self, *args, **kwargs):

@@ -50,6 +50,8 @@ class CategoricalDQN(dqn.DQN):
     """DQN over return distributions; ``q_function`` must return a
     DistributionalDiscreteActionValue, ``clip_delta`` is ignored."""
 
+    _recurrent_supported = False
+
     use_fused_loss = True
 
     def _next_distribution(self, exp_batch):

@@ -7,8 +7,9 @@ class DoubleDQN(dqn.DQN):
     action, the target network evaluates it (pfrl/agents/double_dqn.py:12-40)."""
 
     def _next_q(self, exp_batch):
-        next_state = exp_batch["next_state"]
+        # recurrent: both forwards run over the packed next states from the
+        # batch's next_recurrent_state (double_dqn.py:15-32)
         with evaluating(self.model):
-            next_qout = self.model(next_state)
-        target_next_qout = self.target_model(next_state)
+            next_qout = self._forward(self.model, exp_batch, "next_state")
+        target_next_qout = self._forward(self.target_model, exp_batch, "next_state")
         return target_next_qout.evaluate_actions(next_qout.greedy_actions)

@@ -16,6 +16,8 @@ class AbstractDPP(DQN, metaclass=ABCMeta):
     (an action value -> a [B] tensor); DPP, DPPL and DPPGreedy run it fused on
     CUDA, any other subclass in torch."""
 
+    _recurrent_supported = False
+
     _fused_mode = None
 
     @abstractmethod

@@ -13,8 +13,13 @@ the work happens:
   loss / q statistics: D2H every update      device ring buffers, read lazily
                                                in get_statistics()
 
-Recurrent models, episodic replay and the actor-learner mode are out of scope
-(SURVEY.md section 2).
+With ``recurrent=True`` (DQN and DoubleDQN) the model is a recurrent module
+(``pfrl_b200.nn.RecurrentSequential`` ...) and updates come from episodes
+(``update_from_episodes``).  Acting keeps the batched recurrent states on the
+device, and the transitions handed to the device ``EpisodicReplayBuffer`` carry
+detached device slices of them, so states never leave the GPU; a host buffer
+gets numpy copies, as in the reference (dqn.py:533-545).  The actor-learner
+mode is out of scope (SURVEY.md section 2).
 """
 import collections
 import copy
@@ -24,14 +29,21 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from pfrl_b200 import agent
+from pfrl_b200 import _lib, agent
 from pfrl_b200.ops import losses as fused
-from pfrl_b200.replay_buffer import ReplayUpdater, batch_experiences
+from pfrl_b200.replay_buffer import (
+    AbstractEpisodicReplayBuffer, ReplayUpdater, batch_experiences, batch_recurrent_experiences,
+)
 from pfrl_b200.replay_buffers import PrioritizedReplayBuffer
+from pfrl_b200.replay_buffers.episodic import DeviceEpisodes, EpisodicReplayBuffer
 from pfrl_b200.utils import clip_l2_grad_norm_
 from pfrl_b200.utils.batch_states import batch_states
 from pfrl_b200.utils.modes import evaluating
 from pfrl_b200.utils.copy_param import synchronize_parameters
+from pfrl_b200.utils.recurrent import (
+    get_recurrent_state_at, mask_recurrent_state_at, one_step_forward, pack_and_forward,
+    recurrent_state_as_numpy,
+)
 
 
 def compute_value_loss(y, t, clip_delta=True, batch_accumulator="mean"):
@@ -59,8 +71,23 @@ def compute_weighted_value_loss(y, t, weights, clip_delta=True, batch_accumulato
     return loss_sum / y.shape[0] if batch_accumulator == "mean" else loss_sum
 
 
+def _batch_reset_recurrent_states_when_episodes_end(batch_done, batch_reset, recurrent_states):
+    """Zero the recurrent state of every env whose episode ended (done or reset)."""
+    ended = [i for i, (done, reset) in enumerate(zip(batch_done, batch_reset)) if done or reset]
+    if ended:
+        return mask_recurrent_state_at(recurrent_states, ended)
+    return recurrent_states
+
+
 def make_target_model_as_copy(model):
     target = copy.deepcopy(model)
+
+    def flatten(mod):
+        # cuDNN RNN weights must be made contiguous again after a deep copy
+        if isinstance(mod, torch.nn.RNNBase):
+            mod.flatten_parameters()
+
+    target.apply(flatten)
     target.eval()
     return target
 
@@ -118,6 +145,10 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
 
     saved_attributes = ("model", "target_model", "optimizer")
 
+    # recurrent=True is implemented by DQN and DoubleDQN; the subclasses that
+    # change the target (distributional, quantile, advantage learning) refuse it
+    _recurrent_supported = True
+
     def __init__(self, q_function, optimizer, replay_buffer, gamma, explorer, gpu=None,
                  replay_start_size=50000, minibatch_size=32, update_interval=1,
                  target_update_interval=10000, clip_delta=True, phi=lambda x: x,
@@ -125,8 +156,12 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
                  batch_accumulator="mean", episodic_update_len=None,
                  logger=getLogger(__name__), batch_states=batch_states, recurrent=False,
                  max_grad_norm=None, grad_sync=None, cuda_graph=False):
-        if recurrent:
-            raise NotImplementedError("recurrent DQN is out of scope of pfrl_b200")
+        if recurrent and not self._recurrent_supported:
+            raise NotImplementedError(
+                "recurrent=True is not implemented for %s" % type(self).__name__)
+        if recurrent and (cuda_graph or grad_sync is not None):
+            raise ValueError("recurrent=True cannot be combined with cuda_graph or grad_sync: "
+                             "the packed shapes change with every update")
         self.model = q_function
         if gpu is not None and gpu >= 0:
             assert torch.cuda.is_available()
@@ -148,10 +183,18 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
         assert batch_accumulator in ("mean", "sum")
         self.logger = logger
         self.batch_states = batch_states
-        self.recurrent = False
+        self.recurrent = bool(recurrent)
+        if self.recurrent:
+            assert isinstance(replay_buffer, AbstractEpisodicReplayBuffer)
+            if isinstance(replay_buffer, EpisodicReplayBuffer) and minibatch_size > _lib.SEQ_MAX_B:
+                raise ValueError("the device EpisodicReplayBuffer gathers at most %d sequences "
+                                 "per update (minibatch_size=%d)" % (_lib.SEQ_MAX_B,
+                                                                     minibatch_size))
         self.replay_updater = ReplayUpdater(
-            replay_buffer=replay_buffer, update_func=self.update, batchsize=minibatch_size,
-            episodic_update=False, episodic_update_len=episodic_update_len,
+            replay_buffer=replay_buffer,
+            update_func=self.update_from_episodes if self.recurrent else self.update,
+            batchsize=minibatch_size,
+            episodic_update=self.recurrent, episodic_update_len=episodic_update_len,
             n_times_update=n_times_update, replay_start_size=replay_start_size,
             update_interval=update_interval)
         self.replay_updater.agent = self
@@ -173,6 +216,9 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
         self.loss_record = _DeviceRing(100)
         self.batch_last_obs = []
         self.batch_last_action = []
+        self.train_recurrent_states = None
+        self.train_prev_recurrent_states = None
+        self.test_recurrent_states = None
         # Optional: replay forward(s) + fused loss + backward + clip + optimizer
         # step as ONE CUDA graph (pays off when the minibatch is small and the
         # update is launch-bound, e.g. Nature-DQN at batch 32).
@@ -285,9 +331,18 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
         self._last_q = self._static_q
         return self._static_out
 
+    def _forward(self, model, exp_batch, key):
+        """Q-values of exp_batch[key] ("state" / "next_state"); a recurrent model
+        runs over the packed sequences from the batch's matching initial state."""
+        if not self.recurrent:
+            return model(exp_batch[key])
+        rs = exp_batch["recurrent_state" if key == "state" else "next_recurrent_state"]
+        qout, _ = pack_and_forward(model, exp_batch[key], rs)
+        return qout
+
     def _next_q(self, exp_batch):
         """Value of the next state used in the target: max_a Q_target(s', a)."""
-        return self.target_model(exp_batch["next_state"]).max
+        return self._forward(self.target_model, exp_batch, "next_state").max
 
     def _compute_target_values(self, exp_batch):
         return exp_batch["reward"] + exp_batch["discount"] * (
@@ -295,7 +350,7 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
 
     def _compute_y_and_t(self, exp_batch):
         batch_size = exp_batch["reward"].shape[0]
-        qout = self.model(exp_batch["state"])
+        qout = self._forward(self.model, exp_batch, "state")
         batch_q = torch.reshape(qout.evaluate_actions(exp_batch["action"]), (batch_size, 1))
         with torch.no_grad():
             batch_q_target = torch.reshape(self._compute_target_values(exp_batch), (batch_size, 1))
@@ -308,7 +363,7 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
         if self.use_fused_loss and exp_batch["reward"].is_cuda:
             # one fused kernel: gather Q(s)[a], TD target, |y - t|, Huber / MSE,
             # importance weights and the deterministic batch reduction
-            qout = self.model(exp_batch["state"])
+            qout = self._forward(self.model, exp_batch, "state")
             with torch.no_grad():
                 next_q = self._next_q(exp_batch)
             loss, delta, y, _ = fused.td_loss(
@@ -340,7 +395,17 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
 
     # --------------------------------------------------------------- act/observe
     def _evaluate_model(self, batch_obs):
-        return self.model(self.batch_states(batch_obs, self.device, self.phi))
+        batch_xs = self.batch_states(batch_obs, self.device, self.phi)
+        if not self.recurrent:
+            return self.model(batch_xs)
+        if self.training:
+            self.train_prev_recurrent_states = self.train_recurrent_states
+            batch_av, self.train_recurrent_states = one_step_forward(
+                self.model, batch_xs, self.train_recurrent_states)
+        else:
+            batch_av, self.test_recurrent_states = one_step_forward(
+                self.model, batch_xs, self.test_recurrent_states)
+        return batch_av
 
     def _greedy_graphed(self, batch_obs):
         """Acting forward (a few dozen tiny launches at num_envs images) replayed as one CUDA
@@ -406,27 +471,68 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
                 self.sync_target_network()
             if self.batch_last_obs[i] is not None:
                 assert self.batch_last_action[i] is not None
+                extra = {}
+                if self.recurrent:
+                    extra = dict(
+                        recurrent_state=self._stored_state(self.train_prev_recurrent_states, i),
+                        next_recurrent_state=self._stored_state(self.train_recurrent_states, i))
                 self.replay_buffer.append(
                     state=self.batch_last_obs[i], action=self.batch_last_action[i],
                     reward=batch_reward[i], next_state=batch_obs[i], next_action=None,
-                    is_state_terminal=batch_done[i], env_id=i)
+                    is_state_terminal=batch_done[i], env_id=i, **extra)
                 if batch_reset[i] or batch_done[i]:
                     self.batch_last_obs[i] = None
                     self.batch_last_action[i] = None
                     self.replay_buffer.stop_current_episode(env_id=i)
             self.replay_updater.update_if_necessary(self.t)
+        if self.recurrent:
+            self.train_prev_recurrent_states = None
+            self.train_recurrent_states = _batch_reset_recurrent_states_when_episodes_end(
+                batch_done, batch_reset, self.train_recurrent_states)
+
+    def _stored_state(self, batch_state, i):
+        """State of env i as a transition stores it: a detached device slice for the
+        device episodic buffer (no device-to-host copy), numpy otherwise."""
+        s = get_recurrent_state_at(batch_state, i, detach=True)
+        if isinstance(self.replay_buffer, EpisodicReplayBuffer):
+            return s
+        return recurrent_state_as_numpy(s)
 
     def batch_observe(self, batch_obs, batch_reward, batch_done, batch_reset):
         if self.training:
             return self._batch_observe_train(batch_obs, batch_reward, batch_done, batch_reset)
+        if self.recurrent:
+            if isinstance(batch_done, torch.Tensor):
+                batch_done = batch_done.detach().cpu().numpy()
+            if isinstance(batch_reset, torch.Tensor):
+                batch_reset = batch_reset.detach().cpu().numpy()
+            self.test_recurrent_states = _batch_reset_recurrent_states_when_episodes_end(
+                batch_done, batch_reset, self.test_recurrent_states)
         return None
 
     # ------------------------------------------------------------------- misc
     def stop_episode(self):
-        """Nothing to forget between episodes without recurrent state (dqn.py:791-793)."""
+        """Forget the evaluation recurrent state (dqn.py:790-792)."""
+        if self.recurrent:
+            self.test_recurrent_states = None
 
     def update_from_episodes(self, episodes, errors_out=None):
-        raise NotImplementedError("episodic (recurrent) updates are out of scope of pfrl_b200")
+        """One gradient step from sampled episodes (dqn.py:367-386): sort them by
+        length (stable, longest first), batch them packed, loss, optimizer step.
+        The loss is the scalar TD loss over the packed rows (the fused kernel on
+        CUDA, as in ``update``)."""
+        assert errors_out is None, "Recurrent DQN does not support PrioritizedBuffer"
+        if isinstance(episodes, DeviceEpisodes):
+            episodes = episodes.sorted_by_length()
+        else:
+            episodes = sorted(episodes, key=len, reverse=True)
+        exp_batch = batch_recurrent_experiences(
+            episodes, device=self.device, phi=self.phi, gamma=self.gamma,
+            batch_states=self.batch_states)
+        loss, _ = self._learn(exp_batch, want_errors=False)
+        self.loss_record.append(loss.detach())
+        self.q_record.extend(self._last_q)
+        self.optim_t += 1
 
     def save_snapshot(self, dirname):
         self.save(dirname)

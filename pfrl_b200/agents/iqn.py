@@ -83,6 +83,8 @@ class IQN(dqn.DQN):
     quantile_thresholds_N / _N_prime / _K and act_deterministically as in the
     reference (iqn.py:280-287)."""
 
+    _recurrent_supported = False
+
     def __init__(self, *args, **kwargs):
         self.quantile_thresholds_N = kwargs.pop("quantile_thresholds_N", 64)
         self.quantile_thresholds_N_prime = kwargs.pop("quantile_thresholds_N_prime", 64)

@@ -13,6 +13,8 @@ class PAL(dqn.DQN):
     keyword argument (default 0.9).
     """
 
+    _recurrent_supported = False
+
     _fused_mode = "pal"
 
     def __init__(self, *args, **kwargs):

@@ -149,6 +149,61 @@ int b2rl_flush_pending(b2rl_replay *h, cudaStream_t s);
 int b2rl_launch_repair_multi(b2rl_replay *h, int nranges, const long long *first_slot,
                              const long long *count, long long bump_n, cudaStream_t s);
 
+// ---- gather: one piece of one observation part --------------------------------
+// A part is cut in GATHER_SPLIT pieces so that the CTAs of the gathers are short
+// (~17 KB of traffic) and the last, partially filled wave costs little.
+#define GATHER_SPLIT 2
+
+// Ring slot of the record with logical index i (0 = oldest live record).
+__device__ __forceinline__ long long b2rl_logical_slot(const B2rlDevState *st, long long nslots,
+                                                       long long i)
+{
+    return (st->npop + i) & (nslots - 1);
+}
+
+// Copies piece `piece` of the part `src` to output part `dst_part` (counted in
+// parts from `out`), converting it to f32 in U8_TO_F32 mode.  Every thread of the
+// 256-thread CTA turns one 32-bit word (4 pixels) into one 128-bit store, so both
+// the loads and the stores are fully coalesced (k_gather, k_seq_gather).
+__device__ __forceinline__ void b2rl_gather_part_piece(const uint8_t *src, uint8_t *out,
+                                                       size_t dst_part, int part_bytes,
+                                                       int piece, int obs_mode, float sc)
+{
+    if (obs_mode == B2RL_OBS_U8_TO_F32) {
+        const int words = part_bytes / 4;
+        const int per = (words + GATHER_SPLIT - 1) / GATHER_SPLIT;
+        const int w0 = piece * per;
+        const int w1 = min(words, w0 + per);
+        const uint32_t *s4 = reinterpret_cast<const uint32_t *>(src);
+        float4 *d4 = reinterpret_cast<float4 *>(out) + dst_part * words;
+        constexpr int U = 4; // loads in flight per thread
+        for (int base = w0 + threadIdx.x; base < w1; base += U * 256) {
+            uint32_t v[U];
+#pragma unroll
+            for (int i = 0; i < U; i++)
+                if (base + i * 256 < w1) v[i] = __ldg(s4 + base + i * 256);
+#pragma unroll
+            for (int i = 0; i < U; i++) {
+                if (base + i * 256 >= w1) continue;
+                float4 f;
+                f.x = (float)(v[i] & 0xffu) * sc;
+                f.y = (float)((v[i] >> 8) & 0xffu) * sc;
+                f.z = (float)((v[i] >> 16) & 0xffu) * sc;
+                f.w = (float)(v[i] >> 24) * sc;
+                __stcs(d4 + base + i * 256, f);
+            }
+        }
+    } else {
+        const int vecs = part_bytes / 16;
+        const int per = (vecs + GATHER_SPLIT - 1) / GATHER_SPLIT;
+        const int w0 = piece * per;
+        const int w1 = min(vecs, w0 + per);
+        const uint4 *s16 = reinterpret_cast<const uint4 *>(src);
+        uint4 *d16 = reinterpret_cast<uint4 *>(out) + dst_part * vecs;
+        for (int w = w0 + threadIdx.x; w < w1; w += 256) __stcs(d16 + w, __ldg(s16 + w));
+    }
+}
+
 // Kernel launchers implemented in the other TUs.
 // Recompute the ancestors of up to 4 contiguous leaf-node ranges [lo, hi]
 // (inclusive heap indices at the leaf level; modified in place), then add

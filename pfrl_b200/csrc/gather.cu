@@ -38,15 +38,12 @@ struct GatherArgs {
 __device__ __forceinline__ long long gather_slot(const GatherArgs &a, int k)
 {
     if (a.slots) return a.slots[k];
-    return (a.st->npop + a.index[k]) & (a.nslots - 1);
+    return b2rl_logical_slot(a.st, a.nslots, a.index[k]);
 }
 
-// Grid: one CTA per (experience, side, part, piece) -- each part is cut in
-// GATHER_SPLIT pieces so that the CTAs are short (~17 KB of traffic) and the
-// last, partially filled wave costs little; the slot / part-index lookups are
-// done once per CTA.  The first `tail` CTAs additionally emit the scalars.
-#define GATHER_SPLIT 2
-
+// Grid: one CTA per (experience, side, part, piece) (GATHER_SPLIT pieces per
+// part, b2rl_internal.cuh); the slot / part-index lookups are done once per
+// CTA.  The first `tail` CTAs additionally emit the scalars.
 __global__ void __launch_bounds__(256) k_gather(GatherArgs a)
 {
     const int items = a.n * 2 * a.stack * GATHER_SPLIT;
@@ -62,41 +59,8 @@ __global__ void __launch_bounds__(256) k_gather(GatherArgs a)
             const long long slot = gather_slot(a, k);
             const int32_t ps = (side ? a.next_parts : a.state_parts)[slot * a.stack + part];
             const uint8_t *src = a.parts + (size_t)ps * a.part_bytes;
-            if (a.obs_mode == B2RL_OBS_U8_TO_F32) {
-                const int words = a.part_bytes / 4;
-                const int per = (words + GATHER_SPLIT - 1) / GATHER_SPLIT;
-                const int w0 = piece * per;
-                const int w1 = min(words, w0 + per);
-                const uint32_t *s4 = reinterpret_cast<const uint32_t *>(src);
-                float4 *d4 = reinterpret_cast<float4 *>(out) +
-                             ((size_t)k * a.stack + part) * words;
-                const float sc = a.obs_scale;
-                constexpr int U = 4; // loads in flight per thread
-                for (int base = w0 + threadIdx.x; base < w1; base += U * 256) {
-                    uint32_t v[U];
-#pragma unroll
-                    for (int i = 0; i < U; i++)
-                        if (base + i * 256 < w1) v[i] = __ldg(s4 + base + i * 256);
-#pragma unroll
-                    for (int i = 0; i < U; i++) {
-                        if (base + i * 256 >= w1) continue;
-                        float4 f;
-                        f.x = (float)(v[i] & 0xffu) * sc;
-                        f.y = (float)((v[i] >> 8) & 0xffu) * sc;
-                        f.z = (float)((v[i] >> 16) & 0xffu) * sc;
-                        f.w = (float)(v[i] >> 24) * sc;
-                        __stcs(d4 + base + i * 256, f);
-                    }
-                }
-            } else {
-                const int vecs = a.part_bytes / 16;
-                const int per = (vecs + GATHER_SPLIT - 1) / GATHER_SPLIT;
-                const int w0 = piece * per;
-                const int w1 = min(vecs, w0 + per);
-                const uint4 *s16 = reinterpret_cast<const uint4 *>(src);
-                uint4 *d16 = reinterpret_cast<uint4 *>(out) + ((size_t)k * a.stack + part) * vecs;
-                for (int w = w0 + threadIdx.x; w < w1; w += 256) __stcs(d16 + w, __ldg(s16 + w));
-            }
+            b2rl_gather_part_piece(src, out, (size_t)k * a.stack + part, a.part_bytes, piece,
+                                   a.obs_mode, a.obs_scale);
         }
     }
     // scalar tail: one thread per experience

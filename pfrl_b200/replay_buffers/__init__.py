@@ -3,3 +3,6 @@ from pfrl_b200.replay_buffers.device_buffer import PrioritizedReplayBuffer  # NO
 from pfrl_b200.replay_buffers.device_buffer import PriorityWeightError  # NOQA
 from pfrl_b200.replay_buffers.device_buffer import ReplayBuffer  # NOQA
 from pfrl_b200.replay_buffers.host import HostReplayBuffer  # NOQA
+from pfrl_b200.replay_buffers.episodic import DeviceEpisodes  # NOQA
+from pfrl_b200.replay_buffers.episodic import EpisodicReplayBuffer  # NOQA
+from pfrl_b200.replay_buffers.host import HostEpisodicReplayBuffer  # NOQA

@@ -262,6 +262,55 @@ class DeviceReplayStore:
         res["action"] = res["action"].view((n,) + tuple(action_shape))
         return res
 
+    def gather_sequences(self, first, length, end, obs_mode=OBS_RAW, obs_scale=1.0,
+                         action_dtype=torch.int64, states=None):
+        """Packed minibatch of B sequences (b2rl_replay_gather_sequences).
+        first / length / end: host int arrays, lengths sorted longest first.
+        states: None or (ring, present, leaves) with leaves a list of
+        (offset, d0, inner) -- the state outputs are then [d0, B, inner] f32.
+        Returns a dict of flat packed tensors (rows in pack_sequence order),
+        plus "state_leaves" / "next_state_leaves" lists when states are given."""
+        first = np.ascontiguousarray(first, dtype=np.int64)
+        length = np.ascontiguousarray(length, dtype=np.int32)
+        end = np.ascontiguousarray(end, dtype=np.int64)
+        B = int(first.shape[0])
+        N = int(length.sum())
+        dev = self.device
+        obs_bytes = self.stack * self.part_bytes
+        odt = torch.float32 if obs_mode == OBS_U8_TO_F32 else torch.uint8
+        out = {
+            "state": torch.empty((N, obs_bytes), dtype=odt, device=dev),
+            "next_state": torch.empty((N, obs_bytes), dtype=odt, device=dev),
+            "action": torch.empty((N, self.action_bytes // _itemsize(action_dtype)),
+                                  dtype=action_dtype, device=dev),
+        }
+        out["reward"], out["is_state_terminal"] = torch.empty(
+            (2, N), dtype=torch.float32, device=dev).unbind(0)
+        so = _lib.SeqOut(state=out["state"].data_ptr(), next_state=out["next_state"].data_ptr(),
+                         action=out["action"].data_ptr(), reward=out["reward"].data_ptr(),
+                         terminal=out["is_state_terminal"].data_ptr())
+        ss = None
+        if states is not None:
+            ring, present, leaves = states
+            assert len(leaves) <= _lib.SEQ_MAX_LEAVES, "at most %d state tensors" % (
+                _lib.SEQ_MAX_LEAVES)
+            ss = _lib.SeqStates(ring=ring.data_ptr(), present=present.data_ptr(),
+                                ring_rows=ring.shape[0], row_floats=ring.shape[2],
+                                n_leaves=len(leaves))
+            out["state_leaves"], out["next_state_leaves"] = [], []
+            for i, (off, d0, inner) in enumerate(leaves):
+                s = torch.empty((d0, B, inner), dtype=torch.float32, device=dev)
+                n = torch.empty((d0, B, inner), dtype=torch.float32, device=dev)
+                ss.offset[i], ss.d0[i], ss.inner[i] = off, d0, inner
+                ss.out_state[i], ss.out_next_state[i] = s.data_ptr(), n.data_ptr()
+                out["state_leaves"].append(s)
+                out["next_state_leaves"].append(n)
+        _lib.check(self.L.b2rl_replay_gather_sequences(
+            self.h, _np_ptr(first), _np_ptr(length), _np_ptr(end), B, int(obs_mode),
+            float(obs_scale), ctypes.byref(so), ctypes.byref(ss) if ss is not None else None,
+            _stream(self.device)))
+        return out
+
     def info(self):
         out = _lib.PerInfo()
         _lib.check(self.L.b2rl_per_get_info(self.h, ctypes.byref(out), _stream(self.device)))

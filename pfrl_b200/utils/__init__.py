@@ -7,3 +7,4 @@ from pfrl_b200.utils.random_seed import set_random_seed  # NOQA
 from pfrl_b200.utils.mode_of_distribution import mode_of_distribution  # NOQA
 from pfrl_b200.utils import copy_param  # NOQA  (the module, as in the reference)
 from pfrl_b200.utils import phi  # NOQA  (ScaleU8 / Identity / AsFloat32: phi objects the gather kernel understands)
+from pfrl_b200.utils import recurrent  # NOQA  (the module, as in the reference)

@@ -20,8 +20,9 @@ CALLABLES = """
 agents.DQN agents.DoubleDQN agents.CategoricalDQN agents.CategoricalDoubleDQN agents.IQN
 agents.AL agents.PAL agents.DoublePAL agents.DPP agents.dpp.DPPL agents.dpp.DPPGreedy
 agents.PPO agents.A2C agents.SoftActorCritic agents.TD3 agents.DDPG
-replay_buffers.ReplayBuffer replay_buffers.PrioritizedReplayBuffer
-replay_buffer.batch_experiences replay_buffer.ReplayUpdater utils.batch_states
+replay_buffers.ReplayBuffer replay_buffers.PrioritizedReplayBuffer replay_buffers.EpisodicReplayBuffer
+nn.RecurrentSequential nn.RecurrentBranched replay_buffer.batch_recurrent_experiences
+replay_buffer.random_subseq replay_buffer.batch_experiences replay_buffer.ReplayUpdater utils.batch_states
 experiments.train_agent_batch experiments.train_agent_batch_with_evaluation
 experiments.train_agent experiments.train_agent_with_evaluation
 experiments.evaluator.Evaluator experiments.LinearInterpolationHook
@@ -46,7 +47,7 @@ METHOD_CLASSES = """
 agents.DQN agents.CategoricalDoubleDQN agents.IQN agents.PPO agents.A2C agents.SoftActorCritic
 agents.AL agents.PAL agents.DoublePAL agents.DPP agents.dpp.DPPL agents.dpp.DPPGreedy
 agents.TD3 agents.DDPG replay_buffers.ReplayBuffer replay_buffers.PrioritizedReplayBuffer
-replay_buffer.ReplayUpdater nn.EmpiricalNormalization nn.FactorizedNoisyLinear
+replay_buffer.ReplayUpdater replay_buffers.EpisodicReplayBuffer nn.EmpiricalNormalization nn.FactorizedNoisyLinear
 envs.MultiprocessVectorEnv envs.SerialVectorEnv wrappers.VectorFrameStack
 action_value.DiscreteActionValue action_value.DistributionalDiscreteActionValue
 action_value.QuantileDiscreteActionValue explorers.LinearDecayEpsilonGreedy explorers.AdditiveOU
@@ -54,8 +55,10 @@ collections.random_access_queue.RandomAccessQueue experiments.evaluator.Evaluato
 """.split()
 
 # methods of the reference that belong to features outside the rebuilt path
-OUT_OF_SCOPE = {"setup_actor_learner_training", "update_from_episodes",
+OUT_OF_SCOPE = {"setup_actor_learner_training",
                 "popleft"}  # PrioritizedBuffer.popleft: episodic buffers only
+# per class: recurrent DDPG is outside the rebuilt path (only DQN / DoubleDQN are recurrent)
+OUT_OF_SCOPE_FOR = {"agents.DDPG": {"update_from_episodes"}}
 
 
 def resolve(root, dotted):
@@ -110,7 +113,8 @@ def main():
     for path in METHOD_CLASSES:
         A, B = resolve(ref, path), resolve(ours, path)
         for name, member in inspect.getmembers(A):
-            if name.startswith("_") or name in OUT_OF_SCOPE:
+            if (name.startswith("_") or name in OUT_OF_SCOPE
+                    or name in OUT_OF_SCOPE_FOR.get(path, ())):
                 continue
             if not hasattr(B, name):
                 print("%s: missing attribute %s" % (path, name))

@@ -12,7 +12,7 @@ test files unmodified from where they lie.
     python tools/run_reference_tests.py experiments_tests/test_evaluator.py -k batch
 
 Files that test subsystems outside the rebuilt path (async training, recurrent
-models, persistent buffers, ACER/TRPO/..., ALE wrappers) are not in the list.
+PPO, persistent buffers, ACER/TRPO/..., ALE wrappers) are not in the list.
 """
 import os
 import subprocess
@@ -43,6 +43,8 @@ DEFAULT = [
     "agents_tests/test_ddpg.py",
     "agents_tests/test_al.py", "agents_tests/test_pal.py", "agents_tests/test_double_pal.py",
     "agents_tests/test_dpp.py",
+    "nn_tests/test_recurrent_sequential.py", "nn_tests/test_recurrent_branched.py",
+    "utils_tests/test_recurrent.py",
 ]
 
 PLUGIN = '''
@@ -75,7 +77,8 @@ for name, mod in list(sys.modules.items()):
         mod.__getattr__ = _out_of_scope(name)
 
 from fake_store import OracleBackedStore
-mock.patch("pfrl_b200.replay_buffers.device_buffer.DeviceReplayStore", OracleBackedStore).start()
+from fake_episodic_store import EpisodicOracleStore
+mock.patch("pfrl_b200.replay_buffers.device_buffer.DeviceReplayStore", EpisodicOracleStore).start()
 mock.patch("pfrl_b200.collections.prioritized.DeviceReplayStore", OracleBackedStore).start()
 mock.patch("torch.cuda.current_device", return_value=0).start()
 
