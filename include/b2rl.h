@@ -190,6 +190,13 @@ int b2rl_per_get_info(b2rl_replay *h, b2rl_per_info *out_host, void *stream);
 int b2rl_per_read_priorities(b2rl_replay *h, int64_t first, int64_t n,
                              double *out_host, void *stream);
 
+/* Read heap nodes [first_node, first_node+n) of the sum tree (which = 0) or
+ * the min tree (which = 1) into out_host, after any pending write-back
+ * (synchronises). Node 1 is the root, the leaves of ring slots 0..2P-1 are
+ * nodes 2P..4P-1, node 0 is unused. Test helper. */
+int b2rl_per_read_tree(b2rl_replay *h, int which, int64_t first_node, int64_t n,
+                       double *out_host, void *stream);
+
 /* Restore max_priority when a checkpoint is loaded: the reference pickles the
  * whole PrioritizedBuffer, max_priority included (pfrl/replay_buffers/
  * replay_buffer.py:85-94; pfrl/collections/prioritized.py:32). Synchronises. */

@@ -70,6 +70,12 @@ def lib():
             getattr(L, name).restype = c_i64
             getattr(L, name).argtypes = [vp]
         L.ora_per_append.argtypes = [vp, c_dbl]
+        L.ora_per_append_n.argtypes = [vp, c_i64, vp]
+        L.ora_per_read_tree.argtypes = [vp, ctypes.c_int, c_i64, c_i64, vp]
+        L.ora_per_find.argtypes = [vp, c_i64, vp, vp]
+        L.ora_per_write.argtypes = [vp, c_i64, vp, vp]
+        L.ora_per_live_prefix.restype = c_i64
+        L.ora_per_live_prefix.argtypes = [vp, c_i64, vp]
         L.ora_per_popleft.argtypes = [vp]
         L.ora_per_sample.restype = ctypes.c_int
         L.ora_per_sample.argtypes = [vp, c_i64, vp, vp, vp, vp, vp]

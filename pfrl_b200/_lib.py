@@ -193,6 +193,7 @@ SIGNATURES = {
     "b2rl_per_update_errors": (_int, [_vp, _vp, _int, _i32, _dbl, _dbl, _dbl, _dbl, _vp]),
     "b2rl_per_get_info": (_int, [_vp, ctypes.POINTER(PerInfo), _vp]),
     "b2rl_per_read_priorities": (_int, [_vp, _i64, _i64, _vp, _vp]),
+    "b2rl_per_read_tree": (_int, [_vp, _int, _i64, _i64, _vp, _vp]),
     "b2rl_per_set_max_priority": (_int, [_vp, _dbl, _vp]),
     "b2rl_replay_step": (_int, [_vp, ctypes.POINTER(StepArgs), _vp]),
     "b2rl_step_times": (_int, [_vp, _vp, _vp]),

@@ -70,7 +70,10 @@ __global__ void __launch_bounds__(256) k_gather(GatherArgs a)
     const int len = a.len[slot];
     if (a.o_reward) {
         // sum((gamma**i) * r_i) evaluated like CPython's float sum():
-        // Neumaier-compensated accumulation (replay_buffer.py:183-190)
+        // Neumaier-compensated accumulation (replay_buffer.py:183-190); the
+        // compensation is added only when it is finite, so an infinite or
+        // overflowed sum stays +-inf instead of becoming NaN (CPython also skips
+        // c == 0, which changes nothing here: s starts at +0.0, never becomes -0.0)
         double s = 0.0, c = 0.0;
         for (int i = 0; i < len; i++) {
             const double x = __dmul_rn(a.gamma_pow[i], a.rewards[slot * a.n_step + i]);
@@ -81,7 +84,7 @@ __global__ void __launch_bounds__(256) k_gather(GatherArgs a)
                 c = __dadd_rn(c, __dadd_rn(__dsub_rn(x, t), s));
             s = t;
         }
-        a.o_reward[k] = (float)__dadd_rn(s, c);
+        a.o_reward[k] = (float)(fabs(c) < INFINITY ? __dadd_rn(s, c) : s);
     }
     if (a.o_terminal) a.o_terminal[k] = a.terminal[slot] ? 1.0f : 0.0f;
     if (a.o_discount) a.o_discount[k] = (float)a.gamma_pow[len]; // gamma ** len(elem), :203

@@ -260,10 +260,9 @@ __global__ void __launch_bounds__(1024) k_update(UpdateArgs a)
     if (a.err) {
         // priority_from_errors, replay_buffers/prioritized.py:47-55
         for (int k = tid; k < a.n; k += nt) {
-            double d = a.err_is_f64 ? ((const double *)a.err)[k] : (double)((const float *)a.err)[k];
-            if (a.emin <= a.emax) d = fmin(fmax(d, a.emin), a.emax);
-            d += a.eps;
-            a.new_prio[k] = (a.alpha == 0.5) ? sqrt(d) : pow(d, a.alpha);
+            const double d =
+                a.err_is_f64 ? ((const double *)a.err)[k] : (double)((const float *)a.err)[k];
+            a.new_prio[k] = error_to_priority(d, a.alpha, a.eps, a.emin, a.emax);
         }
     }
     // duplicates: the reference writes in order, so the LAST occurrence wins
@@ -584,6 +583,26 @@ extern "C" int b2rl_per_read_priorities(b2rl_replay *h, int64_t first, int64_t n
                                   cudaMemcpyDeviceToHost, s));
         done += run;
     }
+    B2RL_CUDA(cudaStreamSynchronize(s));
+    return B2RL_OK;
+}
+
+extern "C" int b2rl_per_read_tree(b2rl_replay *h, int which, int64_t first_node, int64_t n,
+                                  double *out, void *stream)
+{
+    B2RL_REQUIRE(h && out, B2RL_ERR_INVALID, "null argument");
+    B2RL_REQUIRE(h->cfg.prioritized, B2RL_ERR_INVALID, "buffer has no priority trees");
+    B2RL_REQUIRE(which == 0 || which == 1, B2RL_ERR_INVALID,
+                 "read_tree: which=%d must be 0 (sum) or 1 (min)", which);
+    B2RL_REQUIRE(first_node >= 0 && n >= 0 && first_node + n <= 2 * h->nslots, B2RL_ERR_RANGE,
+                 "read_tree: nodes [%lld, %lld) outside the heap [0, %lld)", (long long)first_node,
+                 (long long)(first_node + n), (long long)(2 * h->nslots));
+    cudaStream_t s = (cudaStream_t)stream;
+    B2RL_CUDA(cudaSetDevice(h->cfg.device));
+    TRY(b2rl_flush_pending(h, s));
+    if (n > 0)
+        B2RL_CUDA(cudaMemcpyAsync(out, (which ? h->mn : h->sum) + first_node, (size_t)n * 8,
+                                  cudaMemcpyDeviceToHost, s));
     B2RL_CUDA(cudaStreamSynchronize(s));
     return B2RL_OK;
 }

@@ -87,7 +87,10 @@ __device__ __forceinline__ void gather_scalars(const StepGather &g, int k, long 
     const int len = g.len[slot];
     if (g.o_reward) {
         // sum((gamma**i) * r_i) evaluated like CPython's float sum():
-        // Neumaier-compensated accumulation (replay_buffer.py:183-190)
+        // Neumaier-compensated accumulation (replay_buffer.py:183-190); the
+        // compensation is added only when it is finite, so an infinite or
+        // overflowed sum stays +-inf instead of becoming NaN (CPython also skips
+        // c == 0, which changes nothing here: s starts at +0.0, never becomes -0.0)
         double s = 0.0, c = 0.0;
         for (int i = 0; i < len; i++) {
             const double x = __dmul_rn(g.gamma_pow[i], g.rewards[slot * g.n_step + i]);
@@ -98,7 +101,7 @@ __device__ __forceinline__ void gather_scalars(const StepGather &g, int k, long 
                 c = __dadd_rn(c, __dadd_rn(__dsub_rn(x, t), s));
             s = t;
         }
-        g.o_reward[k] = (float)__dadd_rn(s, c);
+        g.o_reward[k] = (float)(fabs(c) < INFINITY ? __dadd_rn(s, c) : s);
     }
     if (g.o_terminal) g.o_terminal[k] = g.terminal[slot] ? 1.0f : 0.0f;
     if (g.o_discount) g.o_discount[k] = (float)g.gamma_pow[len]; // gamma ** len(elem), :203

@@ -776,13 +776,28 @@ __device__ __forceinline__ void upd_stamp(const UpdateArgs &a, int slot)
     }
 }
 
+// (min(hi, max(lo, d)) + eps) ** alpha.  emin > emax: no clipping; an infinite bound is an
+// absent one (DeviceReplayStore passes None as -inf / +inf), so a NaN error is clipped only by
+// a finite bound, as Python's max / min do: max(lo, nan) == lo, min(hi, nan) == hi.  One edge
+// differs: an explicit error_min = -inf with a NaN error gives NaN here, -inf in Python (the
+// priority is then NaN or complex there, which set_last_priority rejects either way).
+__device__ __forceinline__ double error_to_priority(double d, double alpha, double eps,
+                                                    double emin, double emax)
+{
+    if (emin <= emax) {
+        if (emin != -INFINITY) d = fmax(d, emin);
+        if (emax != INFINITY) d = fmin(d, emax);
+    }
+    d += eps;
+    // sqrt is correctly rounded; CUDA's pow(d, 1.0) can be 1 ulp off d, libm's is exact
+    return (alpha == 0.5) ? sqrt(d) : (alpha == 1.0) ? d : pow(d, alpha);
+}
+
 __device__ __forceinline__ double priority_from_error(const UpdateArgs &a, int k)
 {
     // priority_from_errors, replay_buffers/prioritized.py:47-55
     double d = a.err_is_f64 ? ((const double *)a.err)[k] : (double)((const float *)a.err)[k];
-    if (a.emin <= a.emax) d = fmin(fmax(d, a.emin), a.emax);
-    d += a.eps;
-    return (a.alpha == 0.5) ? sqrt(d) : pow(d, a.alpha);
+    return error_to_priority(d, a.alpha, a.eps, a.emin, a.emax);
 }
 
 // The top `topl` <= 10 levels (<= 1023 nodes) recomputed from level `topl` in shared

@@ -327,6 +327,25 @@ class DeviceReplayStore:
         _lib.check(self.L.b2rl_per_read_priorities(self.h, first, n, _np_ptr(out), _stream(self.device)))
         return out
 
+    def read_tree(self, which="sum", first_node=0, n=None):
+        """Heap nodes [first_node, first_node + n) of the sum or min tree as fp64
+        numpy (node 1 is the root, leaves are nodes 2P..4P-1; node 0 is unused)."""
+        w = {"sum": 0, "min": 1}[which]
+        if n is None:
+            n = 2 * self.nslots - first_node
+        out = np.empty(n, dtype=np.float64)
+        _lib.check(self.L.b2rl_per_read_tree(self.h, w, first_node, n, _np_ptr(out),
+                                             _stream(self.device)))
+        return out
+
+    @property
+    def nslots(self):
+        """Leaf slots of the heaps: 2P, P the smallest power of two >= capacity."""
+        p = 1
+        while p < self.capacity:
+            p <<= 1
+        return 2 * p
+
     # -- gather --------------------------------------------------------------
     def gather(self, n, gamma_pow, index=None, obs_mode=OBS_RAW, obs_scale=1.0,
                obs_dtype=None, obs_shape=None, action_dtype=torch.int64,

@@ -31,7 +31,7 @@ CASES = [
     # capacity, kind, n_step, batch, mode, normalize_by_max, prefill
     (300, "frames", 3, 64, "exact", "memory", 500),       # tree in shared memory
     (20000, "vectors", 1, 256, "exact", True, 3000),      # deep tree (D = 3), padded parts
-    (300000, "frames84", 3, 512, "exact", "memory", 9000),  # D = 7, headline frame size
+    (300000, "frames84", 3, 512, "exact", "memory", 9000),  # v6, D = 8, headline frame size
     (600, "frames", 2, 512, "parallel", False, 900),      # with replacement: duplicates
     (5000, "frames", 1, 700, "exact", "batch", 6000),     # batch > 512: write-back alone
     (5000, "frames", 3, 32, "parallel", "memory", 6000),

@@ -22,6 +22,14 @@ V6_CASES = [
     "tests/test_per_gpu.py::test_exact_sampler_deep_trees_bit_identical[70000-3000-2000]",
     "tests/test_per_gpu.py::test_exact_sampler_deep_trees_bit_identical[300000-1500-9000]",
     "tests/test_fused_step_gpu.py::test_fused_step_draws_match_oracle[70000-deep tree]",
+    # adversarial trees at levels 17..21 (v6 D = 5..9, n = 60000 included), stand-alone and fused
+    "tests/test_replay_trees_gpu.py::test_samplers_at_level[17]",
+    "tests/test_replay_trees_gpu.py::test_samplers_at_level[18]",
+    "tests/test_replay_trees_gpu.py::test_samplers_at_level[19]",
+    "tests/test_replay_trees_gpu.py::test_samplers_at_level[20]",
+    "tests/test_replay_trees_gpu.py::test_samplers_at_level[21]",
+    "tests/test_replay_trees_gpu.py::test_npop_at_the_half_boundary[40000-loguniform]",
+    "tests/test_replay_trees_gpu.py::test_npop_at_the_half_boundary[40000-subnormal]",
 ]
 
 
@@ -33,4 +41,4 @@ def test_v6_bit_identity_through_the_slow_path(var, value):
     cmd += ["-m", "pytest", "-q", "-p", "no:cacheprovider"] + V6_CASES
     r = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=1200)
     assert r.returncode == 0, "%s=%s:\n%s\n%s" % (var, value, r.stdout[-4000:], r.stderr[-2000:])
-    assert "3 passed" in r.stdout, r.stdout[-2000:]
+    assert "10 passed" in r.stdout, r.stdout[-2000:]
