@@ -166,7 +166,9 @@ class DeviceNStepBuffer:
         self._pend_exp = []        # (state_slots, next_slots, action, rewards, len, term, prio)
         self._part_head = 0        # sequence number of the next part
         self._part_cache = collections.OrderedDict()  # id(obj) -> (seq, obj)
-        self._live_min_seq = collections.deque()      # per live experience
+        # (experience number, oldest part seq it references): sliding-window minimum
+        # over the live experiences in append order (_note_live)
+        self._live_min_seq = collections.deque()
 
     # -- reference API ------------------------------------------------------
     @property
@@ -294,10 +296,9 @@ class DeviceNStepBuffer:
             hi = min(m, lo + cap)
             self.store.append(sp[lo:hi], nx[lo:hi], np.ascontiguousarray(act[lo:hi]),
                               rw[lo:hi], lens[lo:hi], term[lo:hi])
+        self._note_live(self._n_total, (seq0 + starts).tolist())
         self._n_total += m
-        self._live_min_seq.extend((seq0 + starts).tolist())
-        while len(self._live_min_seq) > cap:
-            self._live_min_seq.popleft()
+        self._check_live_parts()
         return m
 
     _traj_stack = 4
@@ -334,7 +335,8 @@ class DeviceNStepBuffer:
         self._part_cache[key] = (seq, obj)
         if len(self._part_cache) > 8192:
             self._part_cache.popitem(last=False)
-        if len(self._pend_parts) >= 1024:
+        # one upload never holds more parts than the ring (put_parts refuses that)
+        if len(self._pend_parts) >= min(1024, self._part_capacity):
             self._flush_parts()
         return seq
 
@@ -353,16 +355,44 @@ class DeviceNStepBuffer:
         min_seq = min(r[5] for r in window)
         self._pend_exp.append((first[0], last[3], first[1], rewards, len(window), term,
                                self._new_priority()))
+        self._note_live(self._n_total, (min_seq,))
         self._n_total += 1
-        self._live_min_seq.append(min_seq)
-        if len(self._live_min_seq) > self._alloc_capacity:
-            self._live_min_seq.popleft()
         if self._capacity is None and self._n_total > self._alloc_capacity:
             raise MemoryError(
                 "unbounded (capacity=None) device buffer outgrew its %d-experience allocation; "
                 "pass unbounded_capacity=... to reserve more" % self._alloc_capacity)
         if len(self._pend_exp) >= 4096:
             self._flush()
+
+    def _note_live(self, first, seqs):
+        """Experiences number first, first + 1, ... became live; seqs[j] (non-decreasing)
+        is the sequence number of the oldest part that experience first + j references.
+        A later experience can reference an older part than the ones before it (a part
+        reused through the identity cache, e.g. an env that hands out the same reset
+        observation again), so the overrun check needs the minimum over all live
+        experiences, not the oldest experience's: the deque keeps the candidates, seqs
+        non-decreasing front to back."""
+        if not seqs:
+            return
+        q = self._live_min_seq
+        keep = self._alloc_capacity
+        if len(seqs) > keep:  # only the last `capacity` of them stay live
+            first += len(seqs) - keep
+            seqs = seqs[-keep:]
+        while q and q[-1][1] >= seqs[0]:
+            q.pop()
+        q.extend(zip(range(first, first + len(seqs)), seqs))
+        while q[0][0] < first + len(seqs) - keep:
+            q.popleft()  # evicted from the record ring
+
+    def _check_live_parts(self):
+        """MemoryError if a live experience references a part that the ring has already
+        overwritten (sample() would silently return another observation)."""
+        q = self._live_min_seq
+        if q and self._part_head - q[0][1] > self._part_capacity:
+            raise MemoryError(
+                "part ring overrun: live experiences reference parts that were overwritten; "
+                "construct the buffer with a larger part_capacity (now %d)" % self._part_capacity)
 
     def _new_priority(self):
         return None
@@ -397,14 +427,13 @@ class DeviceNStepBuffer:
 
     def _flush(self):
         self._flush_parts()
+        # also with nothing pending: parts uploaded since the last flush may have
+        # overwritten what live experiences reference
+        self._check_live_parts()
         pend = self._pend_exp
         if not pend:
             return
         self._pend_exp = []
-        if self._live_min_seq and self._part_head - self._live_min_seq[0] > self._part_capacity:
-            raise MemoryError(
-                "part ring overrun: live experiences reference parts that were overwritten; "
-                "construct the buffer with a larger part_capacity (now %d)" % self._part_capacity)
         cap = self._alloc_capacity
         lay = self.layout
         for lo in range(0, len(pend), cap):

@@ -105,10 +105,8 @@ def _restore(buf, records, max_priority):
             raise ValueError("a prioritised buffer cannot be restored without priorities")
         buf._pend_exp.append((s_slots, n_slots, act, [float(r) for r in rewards], len(rewards),
                               bool(term), None if priority is None else float(priority)))
+        buf._note_live(buf._n_total, (min(s_min, n_min),))
         buf._n_total += 1
-        buf._live_min_seq.append(min(s_min, n_min))
-        if len(buf._live_min_seq) > buf._alloc_capacity:
-            buf._live_min_seq.popleft()
         if len(buf._pend_exp) >= 4096:
             buf._flush()
     buf._flush()

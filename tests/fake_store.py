@@ -30,6 +30,9 @@ class FakeStore:
 
     def put_parts(self, parts):
         a = np.ascontiguousarray(parts).reshape(-1, self.part_bytes)
+        # b2rl_replay_put_parts refuses more parts than the ring holds
+        assert len(a) <= self.part_capacity, "put_parts: %d parts exceed the ring (%d)" % (
+            len(a), self.part_capacity)
         slots = (self.part_head + np.arange(len(a))) % self.part_capacity
         self.parts[slots] = a
         self.part_head += len(a)
