@@ -283,6 +283,46 @@ int b2rl_replay_gather_sequences(b2rl_replay *h, const int64_t *first_host,
                                  void *stream);
 
 /* ------------------------------------------------------------------------
+ * Sequence gather of a recurrent PPO minibatch (or dataset pass) out of a
+ * time-major rollout [T][E][...]; replaces the per-episode batch_states +
+ * torch.tensor of per-transition scalars + concatenate_recurrent_states +
+ * pack_sequence + H2D of _update_once_recurrent and
+ * _add_log_prob_and_value_to_episodes_recurrent (pfrl/agents/ppo.py:56-107,
+ * 534-606).
+ *
+ * table_host: int64 [first[B]][len[B]][row_off[Lmax + 1]], Lmax = len[0].
+ * Sequence b is env first[b] % E, steps first[b] / E .. + len[b] - 1, so its
+ * step t is the flat slot first[b] + t * E; it is written at the packed row
+ * row_off[t] + b, row_off[t] = sum_b' min(len[b'], t) (pack_sequence order).
+ * Requires len[b] >= 1, len non-increasing (a stable sort, longest first),
+ * first[b] >= 0, first[b] / E + len[b] <= T and the row offsets to be those
+ * of the lengths, else B2RL_ERR_RANGE.  B is not capped.  The table goes to
+ * table_dev (caller-owned, >= table_dev_capacity int64) in one
+ * cudaMemcpyAsync on `stream`: a pinned table_host must stay untouched until
+ * that copy has run.
+ *
+ * cols[c] copies row_bytes bytes of flat slot s of src ([T*E][row_bytes]) to
+ * row r of dst ([N][row_bytes], N = row_off[Lmax]).  index_out (optional)
+ * receives the flat slot of every packed row.  states (optional) is a
+ * b2rl_seq_states whose ring row r is the flat slot r (ring_rows >= T*E): each
+ * sequence's first slot is written to out_state (side 0) / out_next_state
+ * (side 1) of every leaf that has one.  One launch, no synchronisation, no
+ * allocation. */
+#define B2RL_ROLLOUT_MAX_COLS 8
+
+typedef struct {
+    const void *src; /* [T*E][row_bytes] */
+    void *dst;       /* [N][row_bytes]   */
+    int64_t row_bytes;
+} b2rl_rollout_col;
+
+int b2rl_rollout_gather_sequences(const int64_t *table_host, int64_t *table_dev,
+                                  int64_t table_dev_capacity, int32_t B, int64_t T, int64_t E,
+                                  const b2rl_rollout_col *cols, int32_t n_cols,
+                                  int64_t *index_out, const b2rl_seq_states *states,
+                                  void *stream);
+
+/* ------------------------------------------------------------------------
  * Fused replay step: ONE persistent launch per minibatch that
  *   1. writes back the priorities of the PREVIOUS sample if its TD errors were
  *      registered with b2rl_per_defer_errors (set_last_priority,

@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 LIB_PATH = os.path.join(CSRC, "libb2rl.so")
-SOURCES = ["replay.cu", "sampler.cu", "step.cu", "gather.cu", "episodic.cu", "losses.cu", "ppo.cu", "sac.cu", "conv.cu", "gemm.cu"]
+SOURCES = ["replay.cu", "sampler.cu", "step.cu", "gather.cu", "episodic.cu", "rollout.cu", "losses.cu", "ppo.cu", "sac.cu", "conv.cu", "gemm.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
@@ -134,6 +134,14 @@ class SeqStates(ctypes.Structure):
                 ("out_next_state", ctypes.c_void_p * SEQ_MAX_LEAVES)]
 
 
+ROLLOUT_MAX_COLS = 8
+
+
+class RolloutCol(ctypes.Structure):
+    """b2rl_rollout_col (include/b2rl.h)."""
+    _fields_ = [("src", ctypes.c_void_p), ("dst", ctypes.c_void_p), ("row_bytes", ctypes.c_int64)]
+
+
 class GemmOperand(ctypes.Structure):
     """b2rl_gemm_operand (include/b2rl.h)."""
     _fields_ = [("data", ctypes.c_void_p), ("mode", ctypes.c_int32), ("ld", ctypes.c_int32),
@@ -205,6 +213,9 @@ SIGNATURES = {
         _int, [_vp, _vp, _i32, _vp, _int, ctypes.c_float, ctypes.POINTER(BatchOut), _vp]),
     "b2rl_replay_gather_sequences": (
         _int, [_vp, _vp, _vp, _vp, _i32, _int, ctypes.c_float, ctypes.POINTER(SeqOut),
+               ctypes.POINTER(SeqStates), _vp]),
+    "b2rl_rollout_gather_sequences": (
+        _int, [_vp, _vp, _i64, _i32, _i64, _i64, ctypes.POINTER(RolloutCol), _i32, _vp,
                ctypes.POINTER(SeqStates), _vp]),
     "b2rl_c51_loss_fwd": (_int, [_vp] * 7 + [_i32, _i32, _int] + [_vp] * 5),
     "b2rl_c51_loss_bwd": (_int, [_vp] * 4 + [_i32, _i32, _int, _vp, _vp]),

@@ -204,6 +204,54 @@ __device__ __forceinline__ void b2rl_gather_part_piece(const uint8_t *src, uint8
     }
 }
 
+// ---- packed sequences (k_seq_gather, k_rollout_seq_gather) --------------------
+// Step t of packed row `row`: the largest t in [0, Lmax) with row0(t) <= row, where
+// row0(t) = sum_b min(len[b], t) is the packed row of step t of sequence 0
+// (row0(0) = 0, row0(Lmax) = N).  Sequence b = row - row0(t).
+template <class Row0>
+__device__ __forceinline__ int b2rl_packed_step(int row, int Lmax, Row0 row0)
+{
+    int lo = 0, hi = Lmax;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (row0(mid) <= row) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// The recurrent states of each sequence's first record, written by the threads
+// gid, gid + nthreads, ... of the grid: element e of [side][b][float f of the ring row]
+// is float f of side `side` of ring row ring_row(b) (0.0 for a stored None), written
+// into the leaf holding f, laid out [d0][B][inner] (concatenate_recurrent_states).
+// Floats outside every leaf and leaves without an output for that side are skipped.
+// `a` is the kernel's argument block (fields B and rs); reading B from it, not from a
+// copy, keeps k_seq_gather's code as it was before the helper existed.
+template <class Args, class RingRow>
+__device__ __forceinline__ void b2rl_seq_states_write(const Args &a, long long gid,
+                                                      long long nthreads, RingRow ring_row)
+{
+    const b2rl_seq_states &rs = a.rs;
+    const int D = rs.row_floats;
+    const long long total = 2LL * a.B * D;
+    for (long long e = gid; e < total; e += nthreads) {
+        const int side = (int)(e / ((long long)a.B * D));
+        const int rem = (int)(e % ((long long)a.B * D));
+        const int b = rem / D, f = rem % D;
+        int leaf = -1;
+        for (int i = 0; i < rs.n_leaves; i++)
+            if (f >= rs.offset[i] && f < rs.offset[i] + rs.d0[i] * rs.inner[i]) leaf = i;
+        if (leaf < 0) continue;
+        float *out = side ? rs.out_next_state[leaf] : rs.out_state[leaf];
+        if (!out) continue;
+        const long long r = ring_row(b);
+        const float v = rs.present[r * 2 + side] ? rs.ring[(r * 2 + side) * D + f] : 0.0f;
+        const int g = f - rs.offset[leaf];
+        const int inner = rs.inner[leaf];
+        out[((size_t)(g / inner) * a.B + b) * inner + g % inner] = v;
+    }
+}
+
 // Kernel launchers implemented in the other TUs.
 // Recompute the ancestors of up to 4 contiguous leaf-node ranges [lo, hi]
 // (inclusive heap indices at the leaf level; modified in place), then add

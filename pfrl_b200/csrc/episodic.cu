@@ -73,14 +73,8 @@ __global__ void __launch_bounds__(256) k_seq_gather(const __grid_constant__ SeqA
         const int row = (int)(item / (2 * a.stack));
         uint8_t *out = side ? a.o_next : a.o_state;
         if (out) { // uniform over the CTA
-            // step t of the row: the largest t with row0(t) <= row (row0(0) = 0, row0(Lmax) = N)
-            int lo = 0, hi = a.Lmax;
-            while (hi - lo > 1) {
-                const int mid = (lo + hi) >> 1;
-                if (seq_row0_block(a, mid) <= row) lo = mid;
-                else hi = mid;
-            }
-            const int t = lo;
+            const int t =
+                b2rl_packed_step(row, a.Lmax, [&](int u) { return seq_row0_block(a, u); });
             const int b = row - seq_row0_block(a, t);
             const long long slot = b2rl_logical_slot(a.st, a.nslots, a.first[b] + t);
             const int32_t ps = (side ? a.next_parts : a.state_parts)[slot * a.stack + part];
@@ -108,24 +102,9 @@ __global__ void __launch_bounds__(256) k_seq_gather(const __grid_constant__ SeqA
     }
     // recurrent states of each sequence's first record: [side][b][float of the row]
     if (a.has_states) {
-        const int D = a.rs.row_floats;
-        const long long total = 2LL * a.B * D;
-        for (long long e = gid; e < total; e += nthreads) {
-            const int side = (int)(e / ((long long)a.B * D));
-            const int rem = (int)(e % ((long long)a.B * D));
-            const int b = rem / D, f = rem % D;
-            int leaf = -1;
-            for (int i = 0; i < a.rs.n_leaves; i++)
-                if (f >= a.rs.offset[i] && f < a.rs.offset[i] + a.rs.d0[i] * a.rs.inner[i]) leaf = i;
-            if (leaf < 0) continue;
-            float *out = side ? a.rs.out_next_state[leaf] : a.rs.out_state[leaf];
-            if (!out) continue;
-            const long long r = (a.st->npop + a.first[b]) % a.rs.ring_rows;
-            const float v = a.rs.present[r * 2 + side] ? a.rs.ring[(r * 2 + side) * D + f] : 0.0f;
-            const int g = f - a.rs.offset[leaf];
-            const int inner = a.rs.inner[leaf];
-            out[((size_t)(g / inner) * a.B + b) * inner + g % inner] = v;
-        }
+        b2rl_seq_states_write(a, gid, nthreads, [&](int b) {
+            return (a.st->npop + a.first[b]) % a.rs.ring_rows;
+        });
     }
 }
 

@@ -11,8 +11,8 @@ test files unmodified from where they lie.
     python tools/run_reference_tests.py            # the default file list below
     python tools/run_reference_tests.py experiments_tests/test_evaluator.py -k batch
 
-Files that test subsystems outside the rebuilt path (async training, recurrent
-PPO, persistent buffers, ACER/TRPO/..., ALE wrappers) are not in the list.
+Files that test subsystems outside the rebuilt path (async training, persistent
+buffers, ACER/TRPO/..., ALE wrappers) are not in the list.
 """
 import os
 import subprocess
