@@ -1140,16 +1140,25 @@ __device__ __forceinline__ void tree_update_multi(const UpdateArgs &a, unsigned 
 //     blocks.  After a draw of priority p at node o they are updated by plain
 //     subtractions, all entries at once (lanes): M[o], P_lo[e > o in the
 //     block], P_hi[b' > block].  Errors: each entry sees <= n roundings of
-//     <= 2^-53 root, the initial sums <= 80; EPS = (n + 64) 2^-46 root is > 40x
-//     everything a decision depends on (DESIGN.md has the budget).
-//   * bottom 9 levels -> the scout that stages the predicted node's subtree
-//     (exact values, one global round trip, ~4 draws ahead) also lays down the
-//     running sums Q[0..512] of its 512 leaves.
-//   * the main warp decides draw k with
-//         pos12 = u_k * rootA - P_hi[o >> 6] - P_lo[o]   (must be in (EPS, M[o] - EPS))
-//         two 32-way compares of pos12 against Q         (leaf i; pos12 farther
-//                                                         than EPS from Q[i], Q[i+1])
+//     <= 2^-53 root, the initial sums <= 80.
+//   * bottom D levels -> the scout that stages the predicted node's subtree
+//     (exact values, one global round trip, ~4 draws ahead) descends it to a
+//     predicted leaf and lays down a WINDOW of the 32 consecutive leaves around
+//     it: per lane the leaf's lower bound inside the node's interval (the left
+//     siblings on the path to the window's first leaf, top-down, plus an
+//     exclusive warp scan of the window) and its priority, and the window's end.
+//   * the main warp decides draw k with ONE vote against the window, which it
+//     holds in registers (loaded one draw ahead):
+//         pos12 = u_k * rootA - (P_hi[o >> 6] + P_lo[o])  (must be in (EPS, M[o] - EPS))
+//         c = popc(ballot(pos12 >= lo_lane)) - 1          (leaf c of the window; pos12
+//                                                          farther than EPS from lo_c and
+//                                                          from hi_c = lo_c+1 or the end)
 //     and no draw still in flight in the exact pipeline touched that subtree.
+//     Every boundary the reference compares against on the way down lies outside
+//     the leaf's interval, so a pos12 farther than EPS inside it is farther than
+//     EPS from all of them.  The window's bounds add D + 32 roundings; everything
+//     a decision depends on stays within (n + 180) 2^-53 root and EPS =
+//     (n + 64) 2^-46 root is > 45x that for every n >= 1 (DESIGN.md has the budget).
 //     Any doubt (late or wrong scout, margin, conflict) -> SLOW PATH: wait until
 //     the exact tree has caught up and run the reference's arithmetic on it (the
 //     v5 code).  Never wrong, only slow; the count is reported
@@ -1158,31 +1167,40 @@ __device__ __forceinline__ void tree_update_multi(const UpdateArgs &a, unsigned 
 //     global bottom) with the reference's bottom-up adds, one draw after the
 //     other, a few draws behind.  The tree that goes back to HBM and every
 //     priority returned are exact.
-//   * four scout warps; a publisher warp moves results out.
+//   * seven scout warps; a publisher warp moves results out.
 // tools/v6_model.py is a CPU model of the decision logic (adversarial trees:
 // ties, 1e-30..1e+30 dynamic range, u on boundaries, mispredictions).
 // ===========================================================================
-static constexpr int V6_NSCOUT = 4;
-static constexpr int V6_LAG = 4;
-static constexpr int V6_NBUF = 6;
+static constexpr int V6_NSCOUT = 7;
+static constexpr int V6_LAG = 6;
+static constexpr int V6_NBUF = 8;
 static constexpr int V6_Q = 16;
 static constexpr int V6_NTOP = 1 << (V6_T - 1);  // 4096 level-12 nodes
 // Warp roles.  The issue arbiter of an SM sub-partition (warp id % 4) prefers its
 // highest eligible warp id, so the latency-critical main warp gets a sub-partition to
-// itself and all four scouts share another one.
-static constexpr int V6_W_MAIN = 3, V6_W_ASC = 1, V6_W_PUB = 2; // scouts: warps 0, 4, 8, 12
+// itself, the ascent warp shares its own with idle warps only, and the scouts fill
+// sub-partition 0 (warps 0, 4, 8, 12), then sub-partition 2 beside the publisher (warps 6,
+// 10, 14).  Seven scouts, each working on every seventh draw, can start a draw V6_LAG = 6
+// draws ahead; four could not start before they finished the draw four back.
+static constexpr int V6_W_MAIN = 3, V6_W_ASC = 1, V6_W_PUB = 2;
+__device__ __forceinline__ int v6_scout_id(int warp)
+{
+    if ((warp & 3) == 0) return warp >> 2;
+    if ((warp & 3) == 2 && warp != V6_W_PUB) return 3 + (warp >> 2);
+    return -1;
+}
 static constexpr int V6_THREADS = 512;
 
 // One staged subtree: [the 2^(D+1) nodes below a level-12 node, relative heap order: node r
-// has children 2r, 2r+1, leaves at r >= 2^D][QB: exclusive running sums of the 32 nodes five
-// levels down + their total].  The nodes arrive by cp.async.bulk (one copy per level, the
+// has children 2r, 2r+1, leaves at r >= 2^D][the leaf window: 32 lower bounds, 32 priorities,
+// the end, the first leaf (an int)].  The nodes arrive by cp.async.bulk (one copy per level, the
 // level's slice is contiguous in the heap): the copy engine goes global -> shared without
 // touching the SM's L1TEX pipe, which the main warp's shared-memory loads depend on (LDG
 // staging with 32 KB in flight behind a 13 KB L1 made every LDS of the SM wait: ncu showed
 // 330-cycle shared loads).
 __host__ __device__ constexpr size_t v6_buf_doubles(int D)
 {
-    return (size_t(2) << D) + 40;
+    return (size_t(2) << D) + 66;
 }
 
 template <int D>
@@ -1194,38 +1212,6 @@ __host__ __device__ constexpr size_t exact_v6_smem_bytes()
            sizeof(int) * 32 + sizeof(unsigned short) * V6_NTOP + 16 + 8 * V6_NBUF;
 }
 
-// One speculative round of R levels on approximate `pos` (see spec_round): the lane whose
-// comparisons are all consistent wins; `safe` is kept only if every comparison of that lane
-// is farther than eps from equality.
-template <int R>
-__device__ __forceinline__ void spec_round_margin(const double *val, int &node, double &pos,
-                                                  bool &safe, double eps, int lane)
-{
-    if constexpr (R > 0) {
-        const int li = lane & ((1 << R) - 1);
-        double left[R];
-#pragma unroll
-        for (int j = 0; j < R; j++) {
-            const int nj = (node << j) + (li >> (R - j));
-            left[j] = val[2 * nj];
-        }
-        double x = pos;
-        bool ok = true, far = true;
-#pragma unroll
-        for (int j = 0; j < R; j++) {
-            const bool right = (li >> (R - 1 - j)) & 1;
-            const double d = x - left[j];
-            ok = ok && ((d < 0.0) != right);
-            far = far && (fabs(d) > eps);
-            x = right ? d : x;
-        }
-        unsigned m = __ballot_sync(0xffffffffu, ok && far);
-        if constexpr (R < 5) m &= (1u << (1 << R)) - 1u;
-        safe = safe && m != 0;
-        node = (node << R) + (m ? __ffs(m) - 1 : 0);
-    }
-}
-
 template <int D>
 __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_d)
 {
@@ -1235,8 +1221,8 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
     constexpr int SUBN = 2 << D;
     constexpr int NLEAF = 1 << D;               // leaves under one level-12 node
     constexpr int BUFN = (int)v6_buf_doubles(D);
-    constexpr int O_QB = SUBN;                  // [33] running sums of the depth-5 nodes
-    constexpr int R2 = D - 5;                   // levels below the 32-way split
+    // the leaf window: [32] lower bounds, [32] priorities, end, first leaf (relative to 2^D)
+    constexpr int O_WLO = SUBN, O_WPR = SUBN + 32, O_WEND = SUBN + 64, O_WFIRST = SUBN + 65;
     constexpr int PAIRS = (1 << D) - 1;         // child pairs of a whole subtree (slow path)
     constexpr int NIT = (PAIRS + 31) / 32;
     constexpr int CHUNK = 32;
@@ -1251,6 +1237,8 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
     constexpr int F_MAIN = 24, F_ASC = 25, F_PUB = 26, F_ASCR = 27;
     constexpr int ASC_BATCH = 4;
     static_assert(D >= 5 && D <= 9, "v6 stages 5..9 levels per draw");
+    static_assert(NSCOUT >= 1 && NSCOUT <= 7, "scout warps: 0, 4, 8, 12, 6, 10, 14");
+    static_assert(NBUF <= 8, "ready64 has 8 words");
     double *etop = smem_d;                      // exact top, levels 0..12
     double *mtab = etop + TOPN;                 // [NTOP] approximate node mass, descent order
     double *plo = mtab + NTOP;                  // [NTOP] approximate prefix inside a block of 64
@@ -1329,13 +1317,18 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                        (a.dbg_eps_scale > 0.0 ? a.dbg_eps_scale : 1.0);
     __syncthreads();
 
-    if ((warp & 3) == 0 && (warp >> 2) < NSCOUT) {
+    const int sid = v6_scout_id(warp);
+    if (sid >= 0 && sid < NSCOUT) {
         // ------------------------------ scouts -------------------------------
         const double pbar = root0 / (double)(a.st->napp - npop); // expected mass per draw
         long long c_wait = 0, c_fetch = 0, c_rest = 0;
-        for (int k = warp >> 2; k < a.n; k += NSCOUT) {
+        // u of this scout's next draw, loaded one draw ahead: its global latency would
+        // otherwise land on the prediction whenever the wait below is short
+        double u_next = sid < a.n ? a.u[sid] : 0.0;
+        for (int k = sid; k < a.n; k += NSCOUT) {
             const long long tc0 = V6_CLK();
-            const double uk = a.u[k];
+            const double uk = u_next;
+            if (k + NSCOUT < a.n) u_next = a.u[k + NSCOUT];
             const int b = k % NBUF;
             int m;
             while ((m = ld_acquire_smem(&flags[F_MAIN])) < k - LAG ||
@@ -1352,6 +1345,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                     __popc(__ballot_sync(0xffffffffu, pos >= plo[64 * blk + lane + 32])) - 1;
             w = w < 0 ? 0 : w;
             const int ord = 64 * blk + w;
+            pos -= plo[ord];
             const unsigned unode = (unsigned)(NTOP + (ord ^ oflip));
             const int seen = ld_acquire_smem(&flags[F_ASC]);
             double *dst = sub_pref + b * BUFN;
@@ -1366,17 +1360,31 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             const long long tc2 = V6_CLK();
             while (!mbar_try_wait(sb, (uint32_t)((k / NBUF) & 1))) {
             }
-            // ---- running sums of the 32 nodes five levels down (warp scan)
+            // ---- the leaf window: 32 leaves centred on the predicted leaf, clamped to the subtree
             {
-                const double bs = dst[32 + lane];
-                double incl = bs;
+                int r = 1;
+                spec_descend<D>(dst, r, pos, lane);
+                int f = r - NLEAF - 16;
+                f = f < 0 ? 0 : (f > NLEAF - 32 ? NLEAF - 32 : f);
+                // lower bound of leaf f: its left siblings on the path, top-down
+                double base = 0.0;
+#pragma unroll
+                for (int j = D - 1; j >= 0; j--)
+                    if ((f >> j) & 1) base += dst[((NLEAF + f) >> j) - 1];
+                const double p = dst[NLEAF + f + lane];
+                double incl = p;
 #pragma unroll
                 for (int o = 1; o < 32; o <<= 1) {
                     const double up = __shfl_up_sync(0xffffffffu, incl, o);
                     if (lane >= o) incl += up;
                 }
-                dst[O_QB + lane] = incl - bs;
-                if (lane == 31) dst[O_QB + 32] = incl;
+                const double excl = __shfl_up_sync(0xffffffffu, incl, 1);
+                dst[O_WLO + lane] = lane == 0 ? base : base + excl;
+                dst[O_WPR + lane] = p;
+                if (lane == 31) {
+                    dst[O_WEND] = base + incl;
+                    *reinterpret_cast<int *>(&dst[O_WFIRST]) = f;
+                }
             }
             __syncwarp();
             if (lane == 0) {
@@ -1391,7 +1399,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             const long long tc3 = V6_CLK();
             c_wait += tc1 - tc0;
             c_fetch += tc2 - tc1;   // prediction + issue of the loads + store of the internal levels
-            c_rest += tc3 - tc2;    // leaf loads arrive, running sums, stores, release
+            c_rest += tc3 - tc2;    // copy arrives, leaf window, stores, release
         }
         if (a.dbg_cycles && lane == 0 && warp == 0) {
             a.dbg_cycles[8] = c_wait;
@@ -1418,7 +1426,9 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
         int nfast = 0, nslow = 0;
         // prefetched state of the draw about to be decided
         int pf_rs = -1, pf_o = 0, pf_seen = 0, pf_last = 0;
-        double pf_pre = 0.0, pf_mass = 0.0, pf_qb = 0.0;
+        double pf_pre = 0.0, pf_mass = 0.0;
+        double pf_wlo = 0.0, pf_wpr = 0.0, pf_wend = 0.0; // the leaf window, one leaf per lane
+        int pf_wfirst = 0;
         bool pf_stale = false;      // read before the previous draw's stores
         int ord_prev = -1;
         double p_prev = 0.0;
@@ -1439,7 +1449,11 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             pf_pre = phi[pf_o >> 6] + plo[pf_o];
             pf_mass = mtab[pf_o];
             pf_last = lastd[pf_o];
-            pf_qb = sub_pref[b * BUFN + O_QB + lane];
+            const double *w = sub_pref + b * BUFN;
+            pf_wlo = w[O_WLO + lane];
+            pf_wpr = w[O_WPR + lane];
+            pf_wend = w[O_WEND];
+            pf_wfirst = *reinterpret_cast<const int *>(&w[O_WFIRST]);
         };
         if (a.n > 0) prefetch(0);
         for (int k0 = 0; k0 < a.n; k0 += CHUNK) {
@@ -1470,7 +1484,9 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                 // this draw's prefetched state moves to locals; the NEXT draw's loads start now,
                 // behind no store of this warp, and overlap the whole decision below
                 const int c_rs = pf_rs, c_o = pf_o, c_seen = pf_seen, c_last = pf_last;
-                const double c_pre = pf_pre, c_mass = pf_mass, c_qb = pf_qb;
+                const double c_pre = pf_pre, c_mass = pf_mass;
+                const double c_wlo = pf_wlo, c_wpr = pf_wpr, c_wend = pf_wend;
+                const int c_wfirst = pf_wfirst;
                 const bool c_stale = pf_stale;
                 if (k + 1 < a.n) {
                     prefetch(k + 1);
@@ -1489,22 +1505,19 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                     if (c_stale && ord_prev < o) pre -= p_prev; // the update not yet in the tables
                     const double pos = rootA * uk - pre;
                     const double mass = (c_stale && ord_prev == o) ? c_mass - p_prev : c_mass;
-                    const double *sub = sub_pref + b * BUFN;
-                    bool safe = !conflict && pos > eps && pos < mass - eps;
-                    // 32-way compare against the running sums of the nodes five levels down,
-                    // then ONE speculative round over the remaining levels
-                    int blk = __popc(__ballot_sync(0xffffffffu, pos >= c_qb)) - 1;
-                    blk = blk < 0 ? 0 : blk;
-                    const double lo = sub[O_QB + blk], hi = sub[O_QB + blk + 1];
-                    double x = pos - lo;
-                    safe = safe && (x > eps) && (hi - pos > eps);
-                    int r = 32 + blk;
-                    spec_round_margin<R2>(sub, r, x, safe, eps, lane);
-                    const double pr = sub[r];
-                    if (safe) {
+                    // one vote against the window in registers: leaf c, accepted only with pos
+                    // farther than EPS inside [lo_c, hi_c)
+                    const int c = __popc(__ballot_sync(0xffffffffu, pos >= c_wlo)) - 1;
+                    const int cs = c < 0 ? 0 : c;
+                    const double lo = __shfl_sync(0xffffffffu, c_wlo, cs);
+                    const double nx = __shfl_sync(0xffffffffu, c_wlo, (cs + 1) & 31);
+                    const double pr = __shfl_sync(0xffffffffu, c_wpr, cs);
+                    const double hi = cs == 31 ? c_wend : nx;
+                    if (!conflict && c >= 0 && pos > eps && pos < mass - eps && pos - lo > eps &&
+                        hi - pos > eps) {
                         fast = true;
                         ord = o;
-                        rel = r;
+                        rel = NLEAF + c_wfirst + c;
                         prio = pr;
                         nfast++;
                     }
@@ -1550,12 +1563,12 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                     node = NTOP + (ord ^ oflip);
                 }
                 const long long tm2 = V6_CLK();
+                rootA = rootA - prio;
                 // room in the ascent queue: Q entries, checked every fourth draw
                 if ((k & 3) == 0)
                     while (ld_acquire_smem(&flags[F_ASCR]) < k - Q + 4) {
                     }
                 const long long tm3 = V6_CLK();
-                rootA = rootA - prio;
                 // ---- loads first: this draw's table entries
                 const int base = ord & ~63, within = ord & 63, bk = ord >> 6;
                 const double t_m = mtab[ord];
