@@ -2,6 +2,7 @@
 // Not part of the ABI (see include/b2rl.h).
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -65,9 +66,7 @@ struct b2rl_replay {
     int32_t *last_slots;   // [max_batch] slots drawn by the last sample
     double *last_prio;     // [max_batch] their priorities (as found)
     double *new_prio;      // [max_batch] scratch for update
-    double *u_dev;         // [max_batch]
     int32_t *winner;       // [nslots] scratch for duplicate resolution (-1 idle)
-    double *gamma_pow_dev; // [n_step + 1]
     int64_t device_bytes;
 
     // host mirrors
@@ -75,10 +74,9 @@ struct b2rl_replay {
     int64_t part_head; // next part sequence number
     bool wait_priority;
     int last_n;
-    int last_mode;
 
-    // fused replay step (step.cu): cross-CTA "draws ready" counter, launch sequence
-    // number, ring of pinned slots for host-drawn uniforms, deferred write-back
+    // ring of pinned slots for host-drawn uniforms (b2rl_upload_u); fused replay step
+    // (step.cu): cross-CTA "draws ready" counter, launch sequence number; deferred write-back
     unsigned long long *ready_dev;
     unsigned long long *times_dev; // [8 + 256] %globaltimer stamps of the last fused launch
     int last_step_grid;
@@ -141,6 +139,22 @@ struct SampleArgs;
 SampleArgs b2rl_sample_args(const b2rl_replay *h, const double *u, int n, int64_t *index_out,
                             double *prio_user);
 
+// Preconditions of a sample of n draws in `mode` (b2rl_per_sample, b2rl_replay_step): the
+// trees exist, 1 <= n <= max_batch and the live count, no sample awaits its priorities
+// (collections/prioritized.py:98), and every host uniform u_host[i] lies in [0, 1) (u_host
+// null: the uniforms are on the device).  `fn` names the caller in the messages.
+int b2rl_check_sample(const b2rl_replay *h, int n, int mode, const double *u_host, const char *fn);
+
+// Host uniforms u[0..n) to the device through a ring of B2RL_U_RING pinned slots, allocated on
+// first use; *u_dev receives the device copy, valid for the next B2RL_U_RING uploads.
+int b2rl_upload_u(b2rl_replay *h, const double *u, int n, cudaStream_t s, const double **u_dev);
+
+// Write-back arguments for the n priorities of the last sample: in h->new_prio, or computed
+// there from the TD errors `err` (priority_from_errors) when err is not null.
+struct UpdateArgs;
+UpdateArgs b2rl_update_args(const b2rl_replay *h, int n, const void *err, int err_is_f64,
+                            double alpha, double eps, double emin, double emax);
+
 // Apply a write-back registered with b2rl_per_defer_errors (no-op if none).
 int b2rl_flush_pending(b2rl_replay *h, cudaStream_t s);
 
@@ -201,6 +215,66 @@ __device__ __forceinline__ void b2rl_gather_part_piece(const uint8_t *src, uint8
         const uint4 *s16 = reinterpret_cast<const uint4 *>(src);
         uint4 *d16 = reinterpret_cast<uint4 *>(out) + dst_part * vecs;
         for (int w = w0 + threadIdx.x; w < w1; w += 256) __stcs(d16 + w, __ldg(s16 + w));
+    }
+}
+
+// The records, outputs and options of a minibatch gather of n experiences, shared by
+// k_gather (gather.cu) and the gather CTAs of the fused step (step.cu).
+struct GatherArgs {
+    const uint8_t *parts;
+    const int32_t *state_parts, *next_parts;
+    const uint8_t *action;
+    const double *rewards;
+    const uint8_t *len, *terminal;
+    const int32_t *slots;      // slots of the last sample
+    double gamma_pow[9];       // gamma**i, i <= n_step (<= 8), passed by value
+    int n, stack, part_bytes, n_step, action_bytes;
+    int obs_mode;
+    float obs_scale;
+    uint8_t *o_side[2]; // state, next_state (either may be null)
+    uint8_t *o_action;
+    float *o_reward, *o_terminal, *o_discount;
+    double *o_step_rewards;
+    uint8_t *o_len;
+};
+
+GatherArgs b2rl_gather_args(const b2rl_replay *h, int n, const double *gamma_pow_host,
+                            int obs_mode, float obs_scale, const b2rl_batch_out *out);
+
+// Scalars of experience k, stored at ring slot `slot`: n-step reward, discount, terminal,
+// len, step rewards, action (pfrl/replay_buffer.py:183-206).
+__device__ __forceinline__ void b2rl_gather_scalars(const GatherArgs &g, int k, long long slot)
+{
+    const int len = g.len[slot];
+    if (g.o_reward) {
+        // sum((gamma**i) * r_i) evaluated like CPython's float sum():
+        // Neumaier-compensated accumulation (replay_buffer.py:183-190); the
+        // compensation is added only when it is finite, so an infinite or
+        // overflowed sum stays +-inf instead of becoming NaN (CPython also skips
+        // c == 0, which changes nothing here: s starts at +0.0, never becomes -0.0)
+        double s = 0.0, c = 0.0;
+        for (int i = 0; i < len; i++) {
+            const double x = __dmul_rn(g.gamma_pow[i], g.rewards[slot * g.n_step + i]);
+            const double t = __dadd_rn(s, x);
+            if (fabs(s) >= fabs(x))
+                c = __dadd_rn(c, __dadd_rn(__dsub_rn(s, t), x));
+            else
+                c = __dadd_rn(c, __dadd_rn(__dsub_rn(x, t), s));
+            s = t;
+        }
+        g.o_reward[k] = (float)(fabs(c) < INFINITY ? __dadd_rn(s, c) : s);
+    }
+    if (g.o_terminal) g.o_terminal[k] = g.terminal[slot] ? 1.0f : 0.0f;
+    if (g.o_discount) g.o_discount[k] = (float)g.gamma_pow[len]; // gamma ** len(elem), :203
+    if (g.o_len) g.o_len[k] = (uint8_t)len;
+    if (g.o_step_rewards)
+        for (int i = 0; i < g.n_step; i++)
+            g.o_step_rewards[(size_t)k * g.n_step + i] =
+                i < len ? g.rewards[slot * g.n_step + i] : 0.0;
+    if (g.o_action) {
+        const uint8_t *src = g.action + slot * g.action_bytes;
+        uint8_t *dst = g.o_action + (size_t)k * g.action_bytes;
+        for (int i = 0; i < g.action_bytes; i++) dst[i] = src[i];
     }
 }
 

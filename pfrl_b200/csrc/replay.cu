@@ -244,8 +244,6 @@ static int create_impl(b2rl_replay *h)
     TRY(dev_alloc(h, &h->last_slots, (size_t)c.max_batch));
     TRY(dev_alloc(h, &h->last_prio, (size_t)c.max_batch));
     TRY(dev_alloc(h, &h->new_prio, (size_t)c.max_batch));
-    TRY(dev_alloc(h, &h->u_dev, (size_t)c.max_batch));
-    TRY(dev_alloc(h, &h->gamma_pow_dev, (size_t)c.n_step + 1));
     B2RL_CUDA(cudaMemset(h->len, 0, (size_t)h->nslots));
     B2RL_CUDA(cudaMemset(h->terminal, 0, (size_t)h->nslots));
     k_init_state<<<1, 1>>>(h->st);
@@ -311,8 +309,7 @@ extern "C" int b2rl_replay_destroy(b2rl_replay *h)
     cudaDeviceSynchronize();
     void *ptrs[] = {h->parts, h->state_parts, h->next_parts, h->action, h->rewards,
                     h->len, h->terminal, h->sum, h->mn, h->st, h->last_slots,
-                    h->last_prio, h->new_prio, h->u_dev, h->winner, h->gamma_pow_dev,
-                    h->stage};
+                    h->last_prio, h->new_prio, h->winner, h->stage};
     for (void *p : ptrs)
         if (p) cudaFree(p);
     if (h->pin) cudaFreeHost(h->pin);

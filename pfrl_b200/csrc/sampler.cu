@@ -58,11 +58,11 @@ __global__ void __launch_bounds__(512, 1) k_sample_parallel(SampleArgs a)
 static cudaError_t launch_sample(const SampleArgs &a, int mode, cudaStream_t s)
 {
     const SamplerChoice c = choose_sampler(mode, a.levels, a.n);
+    const size_t smem = sampler_smem_bytes(c, a);
     switch (c.kind) {
     case SAMPLER_V6:
         return with_depth<5, 9>(c.D, [&](auto d) {
             constexpr int D = decltype(d)::value;
-            const size_t smem = exact_v6_smem_bytes<D>();
             const cudaError_t e = b2rl_allow_smem<k_sample_exact_v6<D>>(smem);
             if (e != cudaSuccess) return e;
             k_sample_exact_v6<D><<<1, V6_THREADS, smem, s>>>(a);
@@ -71,7 +71,6 @@ static cudaError_t launch_sample(const SampleArgs &a, int mode, cudaStream_t s)
     case SAMPLER_V5:
         return with_depth<1, 10>(c.D, [&](auto d) {
             constexpr int D = decltype(d)::value;
-            const size_t smem = exact_deep_smem_bytes<D>();
             const cudaError_t e = b2rl_allow_smem<k_sample_exact_deep<D>>(smem);
             if (e != cudaSuccess) return e;
             k_sample_exact_deep<D><<<1, 128, smem, s>>>(a);
@@ -80,11 +79,11 @@ static cudaError_t launch_sample(const SampleArgs &a, int mode, cudaStream_t s)
     case SAMPLER_SMALL: {
         const cudaError_t e = b2rl_allow_smem<k_sample_exact>(200 * 1024);
         if (e != cudaSuccess) return e;
-        k_sample_exact<<<1, 256, sizeof(double) * ((size_t(1) << a.T) + (size_t(2) << a.D)), s>>>(a);
+        k_sample_exact<<<1, 256, smem, s>>>(a);
         return cudaGetLastError();
     }
     default:
-        k_sample_parallel<<<1, 512, 64 * sizeof(double), s>>>(a);
+        k_sample_parallel<<<1, 512, smem, s>>>(a);
         return cudaGetLastError();
     }
 }
@@ -134,54 +133,74 @@ SampleArgs b2rl_sample_args(const b2rl_replay *h, const double *u, int n, int64_
     return a;
 }
 
+int b2rl_check_sample(const b2rl_replay *h, int n, int mode, const double *u_host, const char *fn)
+{
+    B2RL_REQUIRE(h->cfg.prioritized, B2RL_ERR_INVALID, "buffer has no priority trees");
+    B2RL_REQUIRE(n > 0 && n <= h->cfg.max_batch, B2RL_ERR_RANGE, "%s: n=%d out of 1..max_batch=%d",
+                 fn, n, h->cfg.max_batch);
+    B2RL_REQUIRE(n <= h->napp - h->npop, B2RL_ERR_RANGE,
+                 "%s: n=%d exceeds the %lld stored experiences", fn, n,
+                 (long long)(h->napp - h->npop));
+    B2RL_REQUIRE(!h->wait_priority, B2RL_ERR_PROTOCOL,
+                 "%s: called again before the previous sample's priorities were set "
+                 "(collections/prioritized.py:98)", fn);
+    B2RL_REQUIRE(mode == B2RL_SAMPLE_EXACT || mode == B2RL_SAMPLE_PARALLEL, B2RL_ERR_INVALID,
+                 "unknown sample mode %d", mode);
+    if (u_host)
+        for (int i = 0; i < n; i++)
+            B2RL_REQUIRE(u_host[i] >= 0.0 && u_host[i] < 1.0, B2RL_ERR_INVALID,
+                         "%s: u[%d]=%g not in [0,1)", fn, i, u_host[i]);
+    return B2RL_OK;
+}
+
+int b2rl_upload_u(b2rl_replay *h, const double *u, int n, cudaStream_t s, const double **u_dev)
+{
+    const int mb = h->cfg.max_batch;
+    if (!h->u_ring_dev) {
+        const size_t ring = (size_t)B2RL_U_RING * mb * sizeof(double);
+        B2RL_CUDA(cudaMallocHost((void **)&h->u_ring_pin, ring));
+        B2RL_CUDA(cudaMalloc((void **)&h->u_ring_dev, ring));
+        for (int i = 0; i < B2RL_U_RING; i++)
+            B2RL_CUDA(cudaEventCreateWithFlags(&h->u_ev[i], cudaEventDisableTiming));
+        h->device_bytes += (int64_t)ring;
+    }
+    // the slot's previous copy (B2RL_U_RING uploads ago) must have left its pinned source
+    const int slot = (int)(h->u_head % B2RL_U_RING);
+    if (h->u_head >= B2RL_U_RING) B2RL_CUDA(cudaEventSynchronize(h->u_ev[slot]));
+    double *pin = h->u_ring_pin + (size_t)slot * mb;
+    double *dev = h->u_ring_dev + (size_t)slot * mb;
+    memcpy(pin, u, (size_t)n * 8);
+    B2RL_CUDA(cudaMemcpyAsync(dev, pin, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+    B2RL_CUDA(cudaEventRecord(h->u_ev[slot], s));
+    h->u_head++;
+    *u_dev = dev;
+    return B2RL_OK;
+}
+
 extern "C" int b2rl_per_sample(b2rl_replay *h, const double *u_host, int32_t n, int mode,
                                int64_t *index_dev, double *priority_dev, void *stream)
 {
     B2RL_REQUIRE(h && u_host, B2RL_ERR_INVALID, "null argument");
-    B2RL_REQUIRE(h->cfg.prioritized, B2RL_ERR_INVALID, "buffer has no priority trees");
-    B2RL_REQUIRE(n > 0 && n <= h->cfg.max_batch, B2RL_ERR_RANGE, "sample: n=%d out of 1..max_batch=%d",
-                 n, h->cfg.max_batch);
-    B2RL_REQUIRE(n <= h->napp - h->npop, B2RL_ERR_RANGE,
-                 "sample: n=%d exceeds the %lld stored experiences", n,
-                 (long long)(h->napp - h->npop));
-    B2RL_REQUIRE(!h->wait_priority, B2RL_ERR_PROTOCOL,
-                 "sample() called again before the previous sample's priorities were set "
-                 "(collections/prioritized.py:98)");
-    B2RL_REQUIRE(mode == B2RL_SAMPLE_EXACT || mode == B2RL_SAMPLE_PARALLEL, B2RL_ERR_INVALID,
-                 "unknown sample mode %d", mode);
+    TRY(b2rl_check_sample(h, n, mode, u_host, "sample"));
     cudaStream_t s = (cudaStream_t)stream;
     B2RL_CUDA(cudaSetDevice(h->cfg.device));
-    for (int i = 0; i < n; i++)
-        B2RL_REQUIRE(u_host[i] >= 0.0 && u_host[i] < 1.0, B2RL_ERR_INVALID,
-                     "sample: u[%d]=%g not in [0,1)", i, u_host[i]);
     TRY(b2rl_flush_pending(h, s));
-    TRY(b2rl_stage_acquire(h, (size_t)n * 8));
-    memcpy(h->pin, u_host, (size_t)n * 8);
-    B2RL_CUDA(cudaMemcpyAsync(h->u_dev, h->pin, (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    TRY(b2rl_stage_release(h, s));
+    const double *u_dev;
+    TRY(b2rl_upload_u(h, u_host, n, s, &u_dev));
 
     // weights are a separate call on this path (b2rl_per_weights)
-    B2RL_CUDA(launch_sample(b2rl_sample_args(h, h->u_dev, n, index_dev, priority_dev), mode, s));
+    B2RL_CUDA(launch_sample(b2rl_sample_args(h, u_dev, n, index_dev, priority_dev), mode, s));
     h->wait_priority = true;
     h->last_n = n;
-    h->last_mode = mode;
     return B2RL_OK;
 }
 
 // ---------------------------------------------------------------------------
 // importance-sampling weights
 // ---------------------------------------------------------------------------
-struct WeightArgs {
-    const B2rlDevState *st;
-    const double *prio;
-    int n;
-    double beta;
-    int norm;
-    float *weight;
-    double *prob;
-};
-
-__global__ void __launch_bounds__(1024) k_weights(WeightArgs a)
+// The last sample's probabilities and weights from its priorities (a.prio_out) and the
+// sum-tree and min-tree roots its sampler recorded in a.st.
+__global__ void __launch_bounds__(1024) k_weights(SampleArgs a)
 {
     __shared__ double red[32];
     __shared__ double s_min;
@@ -190,7 +209,7 @@ __global__ void __launch_bounds__(1024) k_weights(WeightArgs a)
     if (a.norm == B2RL_NORM_BATCH) {
         // np.min(probabilities), replay_buffers/prioritized.py:60
         double m = INFINITY;
-        for (int k = threadIdx.x; k < a.n; k += blockDim.x) m = fmin(m, a.prio[k] / total);
+        for (int k = threadIdx.x; k < a.n; k += blockDim.x) m = fmin(m, a.prio_out[k] / total);
         for (int o = 16; o > 0; o >>= 1) m = fmin(m, __shfl_xor_sync(0xffffffffu, m, o));
         if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
         __syncthreads();
@@ -208,12 +227,9 @@ __global__ void __launch_bounds__(1024) k_weights(WeightArgs a)
     }
     const double len = (double)(a.st->napp - a.st->npop);
     for (int k = threadIdx.x; k < a.n; k += blockDim.x) {
-        const double p = a.prio[k] / total; // :79-82 with uniform_ratio == 0
+        const double p = a.prio_out[k] / total; // :79-82 with uniform_ratio == 0
         if (a.prob) a.prob[k] = p;
-        if (a.weight) {
-            const double base = (a.norm == B2RL_NORM_NONE) ? len * p : p / denom;
-            a.weight[k] = (float)pow(base, -a.beta); // :62 / :64
-        }
+        if (a.weight) a.weight[k] = is_weight(p, denom, len, a.beta, a.norm); // :62 / :64
     }
 }
 
@@ -225,7 +241,11 @@ extern "C" int b2rl_per_weights(b2rl_replay *h, double beta, int norm, float *we
                  "weights requested without a pending sample");
     B2RL_REQUIRE(norm >= 0 && norm <= 2, B2RL_ERR_INVALID, "unknown normalisation %d", norm);
     B2RL_CUDA(cudaSetDevice(h->cfg.device));
-    WeightArgs a{h->st, h->last_prio, h->last_n, beta, norm, weight_dev, prob_dev};
+    SampleArgs a = b2rl_sample_args(h, nullptr, h->last_n, nullptr, nullptr);
+    a.weight = weight_dev;
+    a.prob = prob_dev;
+    a.beta = beta;
+    a.norm = norm;
     k_weights<<<1, 1024, 0, (cudaStream_t)stream>>>(a);
     B2RL_CUDA(cudaGetLastError());
     return B2RL_OK;
@@ -257,14 +277,8 @@ __global__ void __launch_bounds__(1024) k_update(UpdateArgs a)
 {
     __shared__ double red[32];
     const int tid = threadIdx.x, nt = blockDim.x;
-    if (a.err) {
-        // priority_from_errors, replay_buffers/prioritized.py:47-55
-        for (int k = tid; k < a.n; k += nt) {
-            const double d =
-                a.err_is_f64 ? ((const double *)a.err)[k] : (double)((const float *)a.err)[k];
-            a.new_prio[k] = error_to_priority(d, a.alpha, a.eps, a.emin, a.emax);
-        }
-    }
+    if (a.err)
+        for (int k = tid; k < a.n; k += nt) a.new_prio[k] = priority_from_error(a, k);
     // duplicates: the reference writes in order, so the LAST occurrence wins
     for (int k = tid; k < a.n; k += nt) atomicMax(&a.winner[a.slots[k]], k);
     __syncthreads();
@@ -329,10 +343,10 @@ __global__ void __launch_bounds__(1024) k_update(UpdateArgs a)
     }
 }
 
-static int launch_update(b2rl_replay *h, int32_t n, const void *err, int err_is_f64, double alpha,
-                         double eps, double emin, double emax, cudaStream_t s)
+UpdateArgs b2rl_update_args(const b2rl_replay *h, int n, const void *err, int err_is_f64,
+                            double alpha, double eps, double emin, double emax)
 {
-    UpdateArgs a;
+    UpdateArgs a{};
     a.sum = h->sum;
     a.mn = h->mn;
     a.st = h->st;
@@ -348,10 +362,14 @@ static int launch_update(b2rl_replay *h, int32_t n, const void *err, int err_is_
     a.n = n;
     a.levels = h->levels;
     a.nslots = h->nslots;
-    a.nranges = 0;
-    a.bump_n = 0;
     a.capacity = h->cfg.capacity;
-    a.stamps = nullptr;
+    return a;
+}
+
+static int launch_update(b2rl_replay *h, int32_t n, const void *err, int err_is_f64, double alpha,
+                         double eps, double emin, double emax, cudaStream_t s)
+{
+    const UpdateArgs a = b2rl_update_args(h, n, err, err_is_f64, alpha, eps, emin, emax);
     if (n <= UPD_MAX) {
         TRY(launch_update_multi(h, a, s));
     } else {
@@ -411,13 +429,7 @@ extern "C" int b2rl_per_update_errors(b2rl_replay *h, const void *err_dev, int e
 int b2rl_launch_repair_multi(b2rl_replay *h, int nranges, const long long *first_slot,
                              const long long *count, long long bump_n, cudaStream_t s)
 {
-    UpdateArgs a;
-    memset(&a, 0, sizeof(a));
-    a.sum = h->sum;
-    a.mn = h->mn;
-    a.st = h->st;
-    a.levels = h->levels;
-    a.nslots = h->nslots;
+    UpdateArgs a = b2rl_update_args(h, 0, nullptr, 0, 0, 0, 0, 0);
     a.nranges = nranges;
     int total = 0;
     for (int r = 0; r < nranges; r++) {
@@ -427,30 +439,36 @@ int b2rl_launch_repair_multi(b2rl_replay *h, int nranges, const long long *first
     }
     a.n = total;
     a.bump_n = bump_n;
-    a.capacity = h->cfg.capacity;
     return launch_update_multi(h, a, s);
 }
 
-// Deferred form: register the TD errors of the last sample; the trees are
-// updated at the head of the next fused step launch (step.cu) or by the next
-// call that reads or writes them, whichever comes first.  err_dev must stay
-// alive (and unchanged) until then.
+// Register the write-back of launch_update's arguments without launching it: the trees are
+// updated at the head of the next fused step launch (step.cu) or by the next call that reads
+// or writes them, whichever comes first.
+static void defer_update(b2rl_replay *h, int32_t n, const void *err, int err_is_f64, double alpha,
+                         double eps, double emin, double emax)
+{
+    h->pending = true;
+    h->pend_err = err;
+    h->pend_is_f64 = err_is_f64;
+    h->pend_n = n;
+    h->pend_alpha = alpha;
+    h->pend_eps = eps;
+    h->pend_emin = emin;
+    h->pend_emax = emax;
+    h->wait_priority = false; // the sample is answered; the write-back is owed
+    h->last_n = 0;
+}
+
+// Deferred form: register the TD errors of the last sample (defer_update).  err_dev must stay
+// alive (and unchanged) until the write-back runs.
 extern "C" int b2rl_per_defer_errors(b2rl_replay *h, const void *err_dev, int err_is_f64,
                                      int32_t n, double alpha, double eps, double error_min,
                                      double error_max)
 {
     TRY(check_update(h, n));
     B2RL_REQUIRE(err_dev, B2RL_ERR_INVALID, "null errors");
-    h->pending = true;
-    h->pend_err = err_dev;
-    h->pend_is_f64 = err_is_f64;
-    h->pend_n = n;
-    h->pend_alpha = alpha;
-    h->pend_eps = eps;
-    h->pend_emin = error_min;
-    h->pend_emax = error_max;
-    h->wait_priority = false; // the sample is answered; the write-back is owed
-    h->last_n = 0;
+    defer_update(h, n, err_dev, err_is_f64, alpha, eps, error_min, error_max);
     return B2RL_OK;
 }
 
@@ -495,13 +513,7 @@ extern "C" int b2rl_per_update_host_errors(b2rl_replay *h, const double *err_hos
     B2RL_CUDA(cudaMemcpyAsync(h->new_prio, h->pin, (size_t)n * 8, cudaMemcpyHostToDevice, s));
     TRY(b2rl_stage_release(h, s));
     if (!defer) return launch_update(h, n, nullptr, 0, 0, 0, 0, 0, s);
-    h->pending = true;
-    h->pend_err = nullptr; // priorities are already in new_prio
-    h->pend_is_f64 = 0;
-    h->pend_n = n;
-    h->pend_alpha = h->pend_eps = h->pend_emin = h->pend_emax = 0.0;
-    h->wait_priority = false; // the sample is answered; the write-back is owed
-    h->last_n = 0;
+    defer_update(h, n, nullptr, 0, 0, 0, 0, 0); // the priorities are already in new_prio
     return B2RL_OK;
 }
 

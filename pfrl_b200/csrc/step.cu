@@ -38,28 +38,6 @@ static constexpr int GS = 8;            // stages of the part ring in shared mem
 static constexpr int PIECE_MAX = 8192;  // parts larger than this are cut in pieces
 static constexpr int STEP_THREADS = 512;
 
-struct StepGather {
-    const uint8_t *parts;
-    const int32_t *state_parts, *next_parts;
-    const uint8_t *action;
-    const double *rewards;
-    const uint8_t *len, *terminal;
-    const int32_t *slots; // slots of the sample drawn by CTA 0 of this launch
-    double gamma_pow[9];
-    int n, stack, part_bytes, n_step, action_bytes;
-    int obs_mode;
-    float obs_scale;
-    int pieces, piece_bytes, stage_stride;
-    uint8_t *o_side[2]; // state, next_state (either may be null)
-    uint8_t *o_action;
-    float *o_reward, *o_terminal, *o_discount;
-    double *o_step_rewards;
-    uint8_t *o_len;
-    const unsigned long long *ready;
-    unsigned long long seq_base;
-    int poll_ns;
-};
-
 struct StepArgs {
     SampleArgs s;
     UpdateArgs u;
@@ -68,7 +46,11 @@ struct StepArgs {
     // %globaltimer stamps of this launch (b2rl_step_times): [0] CTA 0 entry, [1] write-back
     // complete, [2] all draws published, [8 + c] exit of CTA c
     unsigned long long *times;
-    StepGather g;
+    // gather CTAs: the draws come from a.s (slots) as a.s.ready releases them; parts are
+    // copied in `pieces` pieces of piece_bytes through stages of stage_stride bytes
+    GatherArgs g;
+    int pieces, piece_bytes, stage_stride;
+    int poll_ns;
 };
 
 __device__ __forceinline__ unsigned long long global_ns()
@@ -80,67 +62,31 @@ __device__ __forceinline__ unsigned long long global_ns()
 
 extern __shared__ __align__(128) unsigned char smem_raw[];
 
-// scalars of one experience: n-step reward, discount, terminal, action
-// (pfrl/replay_buffer.py:183-206)
-__device__ __forceinline__ void gather_scalars(const StepGather &g, int k, long long slot)
-{
-    const int len = g.len[slot];
-    if (g.o_reward) {
-        // sum((gamma**i) * r_i) evaluated like CPython's float sum():
-        // Neumaier-compensated accumulation (replay_buffer.py:183-190); the
-        // compensation is added only when it is finite, so an infinite or
-        // overflowed sum stays +-inf instead of becoming NaN (CPython also skips
-        // c == 0, which changes nothing here: s starts at +0.0, never becomes -0.0)
-        double s = 0.0, c = 0.0;
-        for (int i = 0; i < len; i++) {
-            const double x = __dmul_rn(g.gamma_pow[i], g.rewards[slot * g.n_step + i]);
-            const double t = __dadd_rn(s, x);
-            if (fabs(s) >= fabs(x))
-                c = __dadd_rn(c, __dadd_rn(__dsub_rn(s, t), x));
-            else
-                c = __dadd_rn(c, __dadd_rn(__dsub_rn(x, t), s));
-            s = t;
-        }
-        g.o_reward[k] = (float)(fabs(c) < INFINITY ? __dadd_rn(s, c) : s);
-    }
-    if (g.o_terminal) g.o_terminal[k] = g.terminal[slot] ? 1.0f : 0.0f;
-    if (g.o_discount) g.o_discount[k] = (float)g.gamma_pow[len]; // gamma ** len(elem), :203
-    if (g.o_len) g.o_len[k] = (uint8_t)len;
-    if (g.o_step_rewards)
-        for (int i = 0; i < g.n_step; i++)
-            g.o_step_rewards[(size_t)k * g.n_step + i] =
-                i < len ? g.rewards[slot * g.n_step + i] : 0.0;
-    if (g.o_action) {
-        const uint8_t *src = g.action + slot * g.action_bytes;
-        uint8_t *dst = g.o_action + (size_t)k * g.action_bytes;
-        for (int i = 0; i < g.action_bytes; i++) dst[i] = src[i];
-    }
-}
-
 struct Unit {
     int k, sidx, part, piece;
 };
 
-__device__ __forceinline__ Unit decode_unit(const StepGather &g, int nsides, long long q)
+__device__ __forceinline__ Unit decode_unit(const StepArgs &a, int nsides, long long q)
 {
     Unit u;
-    u.piece = (int)(q % g.pieces);
-    long long t = q / g.pieces;
-    u.part = (int)(t % g.stack);
-    t /= g.stack;
+    u.piece = (int)(q % a.pieces);
+    long long t = q / a.pieces;
+    u.part = (int)(t % a.g.stack);
+    t /= a.g.stack;
     u.sidx = (int)(t % nsides);
     u.k = (int)(t / nsides);
     return u;
 }
 
 // One gather CTA.  w = worker index in [0, G).
-__device__ __forceinline__ void gather_worker(const StepGather &g, unsigned char *smem, int w, int G)
+__device__ __forceinline__ void gather_worker(const StepArgs &a, unsigned char *smem, int w, int G)
 {
+    const GatherArgs &g = a.g;
     const int tid = threadIdx.x;
     const int lane = tid & 31, warp = tid >> 5;
     const int nwarps = blockDim.x >> 5;
     uint8_t *stage = smem;
-    uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)GS * g.stage_stride);
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)GS * a.stage_stride);
     uint64_t *empty = full + GS;
     int side_of[2];
     int nsides = 0;
@@ -150,9 +96,9 @@ __device__ __forceinline__ void gather_worker(const StepGather &g, unsigned char
     if (nsides == 0) {
         // scalars only: one thread per experience, strided over the workers
         for (long long k = (long long)w * blockDim.x + tid; k < g.n; k += (long long)G * blockDim.x) {
-            while (ld_acquire_gpu(g.ready) <= g.seq_base + (unsigned long long)k)
-                __nanosleep(g.poll_ns);
-            gather_scalars(g, (int)k, __ldcg(g.slots + k));
+            while (ld_acquire_gpu(a.s.ready) <= a.s.seq_base + (unsigned long long)k)
+                __nanosleep(a.poll_ns);
+            b2rl_gather_scalars(g, (int)k, __ldcg(g.slots + k));
         }
         return;
     }
@@ -166,7 +112,7 @@ __device__ __forceinline__ void gather_worker(const StepGather &g, unsigned char
     }
     __syncthreads();
 
-    const int upe = nsides * g.stack * g.pieces; // units per experience
+    const int upe = nsides * g.stack * a.pieces; // units per experience
     const long long total = (long long)g.n * upe;
     const int my_units = total > w ? (int)((total - w + G - 1) / G) : 0;
 
@@ -181,18 +127,18 @@ __device__ __forceinline__ void gather_worker(const StepGather &g, unsigned char
             const int i = base + lane;
             bool progressed = false;
             if (!done_l && i < my_units) {
-                const Unit u = decode_unit(g, nsides, w + (long long)i * G);
-                const unsigned long long need = g.seq_base + (unsigned long long)u.k;
-                if (r <= need) r = ld_acquire_gpu(g.ready);
+                const Unit u = decode_unit(a, nsides, w + (long long)i * G);
+                const unsigned long long need = a.s.seq_base + (unsigned long long)u.k;
+                if (r <= need) r = ld_acquire_gpu(a.s.ready);
                 if (r > need) {
                     const long long slot = __ldcg(g.slots + u.k);
                     const int side = side_of[u.sidx];
                     const int32_t ps =
                         (side ? g.next_parts : g.state_parts)[slot * g.stack + u.part];
-                    const int off = u.piece * g.piece_bytes;
+                    const int off = u.piece * a.piece_bytes;
                     src_l = (unsigned long long)(g.parts + (size_t)ps * g.part_bytes + off);
-                    bytes_l = (unsigned)min(g.piece_bytes, g.part_bytes - off);
-                    if (u.sidx == 0 && u.part == 0 && u.piece == 0) gather_scalars(g, u.k, slot);
+                    bytes_l = (unsigned)min(a.piece_bytes, g.part_bytes - off);
+                    if (u.sidx == 0 && u.part == 0 && u.piece == 0) b2rl_gather_scalars(g, u.k, slot);
                     done_l = true;
                 }
             }
@@ -204,7 +150,7 @@ __device__ __forceinline__ void gather_worker(const StepGather &g, unsigned char
                     const int s = next % GS;
                     if (next >= GS) mbar_wait(&empty[s], ((next / GS) - 1) & 1);
                     mbar_expect_tx(&full[s], bytes);
-                    bulk_g2s(stage + (size_t)s * g.stage_stride, (const void *)src, bytes, &full[s]);
+                    bulk_g2s(stage + (size_t)s * a.stage_stride, (const void *)src, bytes, &full[s]);
                 }
                 next++;
                 progressed = true;
@@ -214,7 +160,7 @@ __device__ __forceinline__ void gather_worker(const StepGather &g, unsigned char
                 base += 32;
                 done_l = false;
             } else if (!progressed) {
-                __nanosleep(g.poll_ns);
+                __nanosleep(a.poll_ns);
             }
         }
     } else {
@@ -222,12 +168,12 @@ __device__ __forceinline__ void gather_worker(const StepGather &g, unsigned char
         const int ct = tid - 32, nct = blockDim.x - 32;
         for (int i = 0; i < my_units; i++) {
             const int s = i % GS;
-            const Unit u = decode_unit(g, nsides, w + (long long)i * G);
-            const int off = u.piece * g.piece_bytes;
-            const int bytes = min(g.piece_bytes, g.part_bytes - off);
+            const Unit u = decode_unit(a, nsides, w + (long long)i * G);
+            const int off = u.piece * a.piece_bytes;
+            const int bytes = min(a.piece_bytes, g.part_bytes - off);
             uint8_t *out = g.o_side[side_of[u.sidx]];
             const size_t obyte = ((size_t)u.k * g.stack + u.part) * g.part_bytes + off;
-            const uint8_t *src = stage + (size_t)s * g.stage_stride;
+            const uint8_t *src = stage + (size_t)s * a.stage_stride;
             mbar_wait(&full[s], (i / GS) & 1);
             if (g.obs_mode == B2RL_OBS_U8_TO_F32) {
                 const int words = bytes >> 2;
@@ -290,7 +236,7 @@ __global__ void __launch_bounds__(STEP_THREADS, 1) k_replay_step(const __grid_co
             sample_parallel(a.s, reinterpret_cast<double *>(smem_raw));
         if (threadIdx.x == 0) a.times[2] = global_ns();
     } else {
-        gather_worker(a.g, smem_raw, blockIdx.x - 1, gridDim.x - 1);
+        gather_worker(a, smem_raw, blockIdx.x - 1, gridDim.x - 1);
     }
     __syncthreads();
     if (threadIdx.x == 0) a.times[8 + blockIdx.x] = global_ns();
@@ -308,24 +254,19 @@ static cudaError_t launch_step_as(const StepArgs &a, int grid, size_t smem, cuda
 static cudaError_t launch_step(const StepArgs &a, int mode, int grid, size_t smem_other,
                                cudaStream_t s)
 {
-    auto mx = [](size_t x, size_t y) { return x > y ? x : y; };
     const SamplerChoice c = choose_sampler(mode, a.s.levels, a.s.n);
+    const size_t sm = sampler_smem_bytes(c, a.s);
+    const size_t smem = sm > smem_other ? sm : smem_other;
     switch (c.kind) {
-    case SAMPLER_PARALLEL:
-        return launch_step_as<0, SAMPLER_PARALLEL>(a, grid, mx(smem_other, 1024), s);
-    case SAMPLER_SMALL: {
-        const size_t sm = sizeof(double) * ((size_t(1) << a.s.T) + 2);
-        return launch_step_as<0, SAMPLER_SMALL>(a, grid, mx(smem_other, sm), s);
-    }
+    case SAMPLER_PARALLEL: return launch_step_as<0, SAMPLER_PARALLEL>(a, grid, smem, s);
+    case SAMPLER_SMALL: return launch_step_as<0, SAMPLER_SMALL>(a, grid, smem, s);
     case SAMPLER_V6:
         return with_depth<5, 9>(c.D, [&](auto d) {
-            constexpr int D = decltype(d)::value;
-            return launch_step_as<D, SAMPLER_V6>(a, grid, mx(smem_other, exact_v6_smem_bytes<D>()), s);
+            return launch_step_as<decltype(d)::value, SAMPLER_V6>(a, grid, smem, s);
         });
     default:
         return with_depth<1, 10>(c.D, [&](auto d) {
-            constexpr int D = decltype(d)::value;
-            return launch_step_as<D, SAMPLER_V5>(a, grid, mx(smem_other, exact_deep_smem_bytes<D>()), s);
+            return launch_step_as<decltype(d)::value, SAMPLER_V5>(a, grid, smem, s);
         });
     }
 }
@@ -333,65 +274,28 @@ static cudaError_t launch_step(const StepArgs &a, int mode, int grid, size_t sme
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-static int step_resources(b2rl_replay *h)
-{
-    if (h->u_ring_dev) return B2RL_OK;
-    const size_t ring = (size_t)B2RL_U_RING * h->cfg.max_batch * sizeof(double);
-    B2RL_CUDA(cudaMallocHost((void **)&h->u_ring_pin, ring));
-    B2RL_CUDA(cudaMalloc((void **)&h->u_ring_dev, ring));
-    for (int i = 0; i < B2RL_U_RING; i++)
-        B2RL_CUDA(cudaEventCreateWithFlags(&h->u_ev[i], cudaEventDisableTiming));
-    int sm = 0;
-    B2RL_CUDA(cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, h->cfg.device));
-    h->sm_count = sm;
-    h->device_bytes += (int64_t)ring;
-    return B2RL_OK;
-}
-
 extern "C" int b2rl_replay_step(b2rl_replay *h, const b2rl_step_args *p, void *stream)
 {
     B2RL_REQUIRE(h && p, B2RL_ERR_INVALID, "null argument");
-    B2RL_REQUIRE(h->cfg.prioritized, B2RL_ERR_INVALID, "buffer has no priority trees");
-    const int n = p->n;
-    B2RL_REQUIRE(n > 0 && n <= h->cfg.max_batch, B2RL_ERR_RANGE,
-                 "step: n=%d out of 1..max_batch=%d", n, h->cfg.max_batch);
-    B2RL_REQUIRE(n <= h->napp - h->npop, B2RL_ERR_RANGE,
-                 "step: n=%d exceeds the %lld stored experiences", n,
-                 (long long)(h->napp - h->npop));
-    B2RL_REQUIRE(!h->wait_priority, B2RL_ERR_PROTOCOL,
-                 "step: the previous sample's priorities were not set "
-                 "(collections/prioritized.py:98)");
-    B2RL_REQUIRE(p->mode == B2RL_SAMPLE_EXACT || p->mode == B2RL_SAMPLE_PARALLEL,
-                 B2RL_ERR_INVALID, "unknown sample mode %d", p->mode);
     B2RL_REQUIRE(p->u && p->gamma_pow_host, B2RL_ERR_INVALID, "step: null u / gamma_pow");
+    const int n = p->n;
+    TRY(b2rl_check_sample(h, n, p->mode, p->u_on_device ? nullptr : p->u, "step"));
     B2RL_REQUIRE(p->norm >= 0 && p->norm <= 2, B2RL_ERR_INVALID, "unknown normalisation %d",
                  p->norm);
     B2RL_REQUIRE(p->obs_mode == B2RL_OBS_RAW || p->obs_mode == B2RL_OBS_U8_TO_F32,
                  B2RL_ERR_INVALID, "unknown obs_mode %d", p->obs_mode);
     cudaStream_t s = (cudaStream_t)stream;
     B2RL_CUDA(cudaSetDevice(h->cfg.device));
-    TRY(step_resources(h));
+    if (!h->sm_count)
+        B2RL_CUDA(cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, h->cfg.device));
     const b2rl_replay_config &c = h->cfg;
 
     // a deferred write-back too large for the in-launch path goes first, alone
     if (h->pending && h->pend_n > UPD_MAX) TRY(b2rl_flush_pending(h, s));
 
-    // uniforms: device pointer, or host values through a ring of pinned slots
+    // uniforms: device pointer, or host values through the ring of pinned slots
     const double *u_dev = p->u;
-    if (!p->u_on_device) {
-        for (int i = 0; i < n; i++)
-            B2RL_REQUIRE(p->u[i] >= 0.0 && p->u[i] < 1.0, B2RL_ERR_INVALID,
-                         "step: u[%d]=%g not in [0,1)", i, p->u[i]);
-        const int slot = (int)(h->u_head % B2RL_U_RING);
-        if (h->u_head >= B2RL_U_RING) B2RL_CUDA(cudaEventSynchronize(h->u_ev[slot]));
-        double *pin = h->u_ring_pin + (size_t)slot * c.max_batch;
-        double *dev = h->u_ring_dev + (size_t)slot * c.max_batch;
-        memcpy(pin, p->u, (size_t)n * 8);
-        B2RL_CUDA(cudaMemcpyAsync(dev, pin, (size_t)n * 8, cudaMemcpyHostToDevice, s));
-        B2RL_CUDA(cudaEventRecord(h->u_ev[slot], s));
-        h->u_head++;
-        u_dev = dev;
-    }
+    if (!p->u_on_device) TRY(b2rl_upload_u(h, p->u, n, s, &u_dev));
 
     StepArgs a;
     memset(&a, 0, sizeof(a));
@@ -416,65 +320,26 @@ extern "C" int b2rl_replay_step(b2rl_replay *h, const b2rl_step_args *p, void *s
     // ---- deferred write-back of the previous sample
     a.upd_n = 0;
     if (h->pending) {
-        a.u.sum = h->sum;
-        a.u.mn = h->mn;
-        a.u.st = h->st;
-        a.u.slots = h->last_slots;
-        a.u.new_prio = h->new_prio;
-        a.u.err = h->pend_err;
-        a.u.err_is_f64 = h->pend_is_f64;
-        a.u.alpha = h->pend_alpha;
-        a.u.eps = h->pend_eps;
-        a.u.emin = h->pend_emin;
-        a.u.emax = h->pend_emax;
-        a.u.winner = h->winner;
-        a.u.n = h->pend_n;
-        a.u.levels = h->levels;
-        a.u.nslots = h->nslots;
+        a.u = b2rl_update_args(h, h->pend_n, h->pend_err, h->pend_is_f64, h->pend_alpha,
+                               h->pend_eps, h->pend_emin, h->pend_emax);
+        a.u.stamps = h->times_dev + 3; // [3..7]: phases of the write-back
         a.upd_n = h->pend_n;
         a.upd_sync = h->ready_dev + 1;
-        a.u.stamps = h->times_dev + 3; // [3..7]: phases of the write-back
     }
     a.times = h->times_dev;
     // ---- gather
-    StepGather &g = a.g;
-    g.parts = h->parts;
-    g.state_parts = h->state_parts;
-    g.next_parts = h->next_parts;
-    g.action = h->action;
-    g.rewards = h->rewards;
-    g.len = h->len;
-    g.terminal = h->terminal;
-    g.slots = h->last_slots;
-    for (int i = 0; i <= c.n_step; i++) g.gamma_pow[i] = p->gamma_pow_host[i];
-    g.n = n;
-    g.stack = c.stack;
-    g.part_bytes = c.part_bytes;
-    g.n_step = c.n_step;
-    g.action_bytes = c.action_bytes;
-    g.obs_mode = p->obs_mode;
-    g.obs_scale = p->obs_scale;
-    g.pieces = (c.part_bytes + PIECE_MAX - 1) / PIECE_MAX;
-    g.piece_bytes = (((c.part_bytes + g.pieces - 1) / g.pieces) + 15) & ~15;
-    g.stage_stride = (g.piece_bytes + 127) & ~127;
-    g.o_side[0] = (uint8_t *)p->out.state;
-    g.o_side[1] = (uint8_t *)p->out.next_state;
-    g.o_action = (uint8_t *)p->out.action;
-    g.o_reward = p->out.reward;
-    g.o_terminal = p->out.terminal;
-    g.o_discount = p->out.discount;
-    g.o_step_rewards = p->out.step_rewards;
-    g.o_len = p->out.len;
-    g.ready = h->ready_dev;
-    g.seq_base = seq_base;
-    g.poll_ns = p->mode == B2RL_SAMPLE_EXACT ? 400 : 100;
+    a.g = b2rl_gather_args(h, n, p->gamma_pow_host, p->obs_mode, p->obs_scale, &p->out);
+    a.pieces = (c.part_bytes + PIECE_MAX - 1) / PIECE_MAX;
+    a.piece_bytes = (((c.part_bytes + a.pieces - 1) / a.pieces) + 15) & ~15;
+    a.stage_stride = (a.piece_bytes + 127) & ~127;
+    a.poll_ns = p->mode == B2RL_SAMPLE_EXACT ? 400 : 100;
 
-    const int nsides = (g.o_side[0] ? 1 : 0) + (g.o_side[1] ? 1 : 0);
-    long long units = nsides ? (long long)n * nsides * c.stack * g.pieces : (n + STEP_THREADS - 1) / STEP_THREADS;
+    const int nsides = (a.g.o_side[0] ? 1 : 0) + (a.g.o_side[1] ? 1 : 0);
+    long long units = nsides ? (long long)n * nsides * c.stack * a.pieces : (n + STEP_THREADS - 1) / STEP_THREADS;
     int grid = h->sm_count;
     if (units + 1 < grid) grid = (int)units + 1;
     if (grid < 2) grid = 2;
-    size_t smem = (size_t)GS * g.stage_stride + 2 * GS * sizeof(uint64_t);
+    size_t smem = (size_t)GS * a.stage_stride + 2 * GS * sizeof(uint64_t);
     if (a.upd_n > 0) {
         const size_t us = update_multi_smem_bytes(h->levels);
         if (us > smem) smem = us;
@@ -484,7 +349,6 @@ extern "C" int b2rl_replay_step(b2rl_replay *h, const b2rl_step_args *p, void *s
     h->pending = false;
     h->wait_priority = true;
     h->last_n = n;
-    h->last_mode = p->mode;
     return B2RL_OK;
 }
 

@@ -215,6 +215,35 @@ __device__ __forceinline__ float is_weight(double prob, double denom, double len
     return (float)pow(base, -beta);
 }
 
+// Outputs of finished draw k (leaf `slot`, priority `prio`): the slot and priority kept for the
+// write-back, the optional logical index and user priority, the probability prio / total and,
+// unless the norm needs the batch minimum, the weight.  bmin takes the minimum probability.
+__device__ __forceinline__ void store_draw(const SampleArgs &a, int k, long long slot, double prio,
+                                           double total, double mroot, double len, long long npop,
+                                           double &bmin)
+{
+    a.slots_out[k] = (int32_t)slot;
+    a.prio_out[k] = prio;
+    if (a.index_out) a.index_out[k] = (slot - npop) & (a.nslots - 1);
+    if (a.prio_user) a.prio_user[k] = prio;
+    const double p = prio / total;
+    if (a.prob) a.prob[k] = p;
+    bmin = fmin(bmin, p);
+    if (a.weight && a.norm != B2RL_NORM_BATCH)
+        a.weight[k] = is_weight(p, mroot / total, len, a.beta, a.norm);
+}
+
+// Weights normalised by the batch's smallest probability bmin (np.min(probabilities),
+// replay_buffers/prioritized.py:60), of draws k0, k0 + stride, ... (the caller's lanes or
+// threads) once every draw is stored; a.norm is B2RL_NORM_BATCH.
+__device__ __forceinline__ void store_batch_weights(const SampleArgs &a, double total, double bmin,
+                                                    double len, int k0, int stride)
+{
+#pragma unroll 1 // one pow in flight: no register cost to the samplers that inline this
+    for (int k = k0; k < a.n; k += stride)
+        a.weight[k] = is_weight(a.prio_out[k] / total, bmin, len, a.beta, a.norm);
+}
+
 // ---------------------------------------------------------------------------
 // speculative lane-parallel descent (see sampler.cu header comment)
 //
@@ -287,8 +316,7 @@ static constexpr int EX_NSCOUT = 2;
 static constexpr int EX_LAG = 2;
 static constexpr int EX_NBUF = EX_LAG + 1;
 
-template <int D>
-__host__ __device__ constexpr size_t exact_deep_smem_bytes()
+constexpr size_t exact_deep_smem_bytes(int D)
 {
     return sizeof(double) * ((size_t(1) << TOP_LEVELS) + (size_t(2) << D) * (1 + EX_NBUF) +
                              EX_RING + 2) +
@@ -495,19 +523,9 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
                 mroot = s_stat[1];
             }
             const int k = k0 + lane;
-            if (k < kend) {
-                const long long slot = o_slot[k % RING];
-                const double prio = o_prio[k % RING];
-                a.slots_out[k] = (int32_t)slot;
-                a.prio_out[k] = prio;
-                if (a.index_out) a.index_out[k] = (slot - npop) & mask;
-                if (a.prio_user) a.prio_user[k] = prio;
-                const double p = prio / total;
-                if (a.prob) a.prob[k] = p;
-                bmin = fmin(bmin, p);
-                if (a.weight && a.norm != B2RL_NORM_BATCH)
-                    a.weight[k] = is_weight(p, mroot / total, len, a.beta, a.norm);
-            }
+            if (k < kend)
+                store_draw(a, k, o_slot[k % RING], o_prio[k % RING], total, mroot, len, npop,
+                           bmin);
             __syncwarp();
             if (lane == 0) {
                 if (a.ready) st_release_gpu(a.ready, a.seq_base | (unsigned long long)kend);
@@ -518,8 +536,7 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
         if (a.weight && a.norm == B2RL_NORM_BATCH) {
             // np.min(probabilities) over the batch, replay_buffers/prioritized.py:60
             for (int o = 16; o > 0; o >>= 1) bmin = fmin(bmin, __shfl_xor_sync(0xffffffffu, bmin, o));
-            for (int k = lane; k < a.n; k += 32)
-                a.weight[k] = is_weight(a.prio_out[k] / total, bmin, len, a.beta, a.norm);
+            store_batch_weights(a, total, bmin, len, lane, 32);
         }
     }
     __syncthreads();
@@ -542,7 +559,6 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
 __device__ __forceinline__ void exact_small(const SampleArgs &a, double *smem_d)
 {
     double *top = smem_d;
-    double *sub = smem_d + (1 << a.T);
     const int topn = 1 << a.T;
     const int tid = threadIdx.x;
     for (int i = 1 + tid; i < topn; i += blockDim.x) top[i] = a.sum[i];
@@ -588,64 +604,20 @@ __device__ __forceinline__ void exact_small(const SampleArgs &a, double *smem_d)
                     node = 2 * node + 1;
                 }
             }
-            long long leafnode;
-            double prio;
-            if (a.D > 0) {
-                // one round trip: all D levels under `node`
-                for (int j = 1; j <= a.D; j++) {
-                    const int cnt = 1 << j;
-                    const double *src = a.sum + ((long long)node << j);
-                    for (int i = lane; i < cnt; i += 32) sub[cnt + i] = src[i];
-                }
-                __syncwarp();
-                int rel = 1;
-                for (int j = 0; j < a.D; j++) {
-                    const double left = sub[2 * rel];
-                    if (pos < left) {
-                        rel = 2 * rel;
-                    } else {
-                        pos = __dsub_rn(pos, left);
-                        rel = 2 * rel + 1;
-                    }
-                }
-                leafnode = ((long long)node << a.D) + (rel - (1 << a.D));
-                prio = sub[rel];
-                // _write(ix, 0.0): zero the leaf, re-reduce the path, :303
-                sub[rel] = 0.0;
-                if (lane == 0) a.sum[leafnode] = 0.0;
-                int dj = a.D - 1;
-                for (int p = rel >> 1; p >= 2; p >>= 1, dj--) {
-                    const double v = __dadd_rn(sub[2 * p], sub[2 * p + 1]);
-                    sub[p] = v;
-                    if (lane == 0) a.sum[((long long)node << dj) + (p - (1 << dj))] = v;
-                }
-                top[node] = __dadd_rn(sub[2], sub[3]);
-            } else {
-                leafnode = node;
-                prio = top[node];
-                top[node] = 0.0;
-            }
+            // the leaves are in shared memory (D == 0): _write(ix, 0.0), :303
+            const double prio = top[node];
+            top[node] = 0.0;
             for (int p = node >> 1; p >= 1; p >>= 1)
                 top[p] = __dadd_rn(top[2 * p], top[2 * p + 1]);
             if (lane == 0) {
-                const long long slot = leafnode - a.nslots;
-                a.slots_out[k] = (int32_t)slot;
-                a.prio_out[k] = prio;
-                if (a.index_out) a.index_out[k] = (slot - npop) & mask;
-                if (a.prio_user) a.prio_user[k] = prio;
-                const double p = prio / total;
-                if (a.prob) a.prob[k] = p;
-                bmin = fmin(bmin, p);
-                if (a.weight && a.norm != B2RL_NORM_BATCH)
-                    a.weight[k] = is_weight(p, mroot / total, len, a.beta, a.norm);
+                store_draw(a, k, node - a.nslots, prio, total, mroot, len, npop, bmin);
                 if (a.ready && ((k & 31) == 31 || k == a.n - 1))
                     st_release_gpu(a.ready, a.seq_base | (unsigned long long)(k + 1));
             }
             __syncwarp();
         }
         if (lane == 0 && a.weight && a.norm == B2RL_NORM_BATCH)
-            for (int k = 0; k < a.n; k++)
-                a.weight[k] = is_weight(a.prio_out[k] / total, bmin, len, a.beta, a.norm);
+            store_batch_weights(a, total, bmin, len, 0, 1);
     }
     __syncthreads();
     // publish the shared-memory levels (zeroed state) back to HBM
@@ -703,16 +675,7 @@ __device__ __forceinline__ void sample_parallel(const SampleArgs &a, double *red
             }
         }
         const double prio = a.sum[node];
-        const long long slot = node - a.nslots;
-        a.slots_out[k] = (int32_t)slot;
-        a.prio_out[k] = prio;
-        if (a.index_out) a.index_out[k] = (slot - npop) & mask;
-        if (a.prio_user) a.prio_user[k] = prio;
-        const double p = prio / root;
-        if (a.prob) a.prob[k] = p;
-        bmin = fmin(bmin, p);
-        if (a.weight && a.norm != B2RL_NORM_BATCH)
-            a.weight[k] = is_weight(p, mroot / root, len, a.beta, a.norm);
+        store_draw(a, k, node - a.nslots, prio, root, mroot, len, npop, bmin);
     }
     if (threadIdx.x == 0) {
         a.st->last_total = root;
@@ -725,8 +688,7 @@ __device__ __forceinline__ void sample_parallel(const SampleArgs &a, double *red
         __syncthreads();
         bmin = INFINITY;
         for (int w = 0; w < (int)(blockDim.x >> 5); w++) bmin = fmin(bmin, red[w]);
-        for (int k = threadIdx.x; k < a.n; k += blockDim.x)
-            a.weight[k] = is_weight(a.prio_out[k] / root, bmin, len, a.beta, a.norm);
+        store_batch_weights(a, root, bmin, len, threadIdx.x, blockDim.x);
     }
     __syncthreads();
     if (threadIdx.x == 0 && a.ready) {
@@ -1203,13 +1165,25 @@ __host__ __device__ constexpr size_t v6_buf_doubles(int D)
     return (size_t(2) << D) + 66;
 }
 
-template <int D>
-__host__ __device__ constexpr size_t exact_v6_smem_bytes()
+constexpr size_t exact_v6_smem_bytes(int D)
 {
     // etop, M, P_lo, P_hi(64) + rootA + stat(2) + pad, sub_own, NBUF x staged buffer, o_prio
     return sizeof(double) * ((size_t(1) << V6_T) + 2 * V6_NTOP + 80 + (size_t(2) << D) +
                              V6_NBUF * v6_buf_doubles(D) + 2 * EX_RING) +
            sizeof(int) * 32 + sizeof(unsigned short) * V6_NTOP + 16 + 8 * V6_NBUF;
+}
+
+// Dynamic shared memory of the sampler `c` serving the draw `a` (launch_sample in sampler.cu,
+// launch_step in step.cu): exact_small holds the whole tree (nodes [1, 2^T)), sample_parallel
+// its per-warp minima.
+inline size_t sampler_smem_bytes(const SamplerChoice &c, const SampleArgs &a)
+{
+    switch (c.kind) {
+    case SAMPLER_PARALLEL: return 64 * sizeof(double);
+    case SAMPLER_SMALL: return sizeof(double) << a.T;
+    case SAMPLER_V6: return exact_v6_smem_bytes(c.D);
+    default: return exact_deep_smem_bytes(c.D);
+    }
 }
 
 template <int D>
@@ -1685,19 +1659,9 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                 mroot = s_misc[2];
             }
             const int k = k0 + lane;
-            if (k < kend) {
-                const long long slot = ring[k % RING].slot;
-                const double prio = ring[k % RING].prio;
-                a.slots_out[k] = (int32_t)slot;
-                a.prio_out[k] = prio;
-                if (a.index_out) a.index_out[k] = (slot - npop) & mask;
-                if (a.prio_user) a.prio_user[k] = prio;
-                const double p = prio / total;
-                if (a.prob) a.prob[k] = p;
-                bmin = fmin(bmin, p);
-                if (a.weight && a.norm != B2RL_NORM_BATCH)
-                    a.weight[k] = is_weight(p, mroot / total, len, a.beta, a.norm);
-            }
+            if (k < kend)
+                store_draw(a, k, ring[k % RING].slot, ring[k % RING].prio, total, mroot, len,
+                           npop, bmin);
             __syncwarp();
             if (lane == 0) {
                 if (a.ready) st_release_gpu(a.ready, a.seq_base | (unsigned long long)kend);
@@ -1707,8 +1671,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
         }
         if (a.weight && a.norm == B2RL_NORM_BATCH) {
             for (int o = 16; o > 0; o >>= 1) bmin = fmin(bmin, __shfl_xor_sync(0xffffffffu, bmin, o));
-            for (int k = lane; k < a.n; k += 32)
-                a.weight[k] = is_weight(a.prio_out[k] / total, bmin, len, a.beta, a.norm);
+            store_batch_weights(a, total, bmin, len, lane, 32);
         }
     }
     __syncthreads();
