@@ -511,7 +511,11 @@ int b2rl_ppo_loss(const float *log_prob, const float *entropy,
  * each operation rounded separately -- bit for bit soft_copy_param's
  * `target.mul_(1 - tau); target.add_(tau * source)` (pfrl/utils/copy_param.py:9-22,
  * called from SoftActorCritic.sync_target_network, soft_actor_critic.py:199-212).
- * pairs_host is read before the call returns. */
+ * pairs_host is read before the call returns.  Every pair needs non-NULL pointers
+ * (an empty pair included) and numel >= 0, and tau must lie in [0, 1]; all of it is
+ * checked before the first launch, so a refused call changes no target.  Pairs
+ * are updated concurrently: no target may share memory with another target or a
+ * source. */
 typedef struct {
     void *dst;       /* target tensor (device, fp32, contiguous) */
     const void *src; /* source tensor (device, fp32, contiguous) */
@@ -523,7 +527,8 @@ int b2rl_polyak(const b2rl_tensor_pair *pairs_host, int32_t n_pairs, double tau,
 /* Entropy-regularised TD target of SoftActorCritic.update_q_func
  * (pfrl/agents/soft_actor_critic.py:225-240):
  *   out = reward + discount * (1 - terminal) * (min(q1, q2) - temperature * log_prob)
- * with the reference's operation order and one rounding per operation.
+ * with the reference's operation order and one rounding per operation; min is
+ * torch.min's: NaN when either Q is NaN.
  * temperature_dev (device scalar) takes precedence over `temperature`. */
 int b2rl_sac_target(const float *reward, const float *discount, const float *terminal,
                     const float *q1, const float *q2, const float *log_prob,

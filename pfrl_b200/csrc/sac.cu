@@ -52,7 +52,9 @@ __global__ void __launch_bounds__(256) k_sac_target(const float *reward, const f
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float alpha = temperature_dev ? *temperature_dev : temperature;
-    const float next_q = fminf(q1[i], q2[i]);                        // torch.min(q1', q2')
+    const float a = q1[i], b = q2[i];
+    // torch.min(q1', q2'): NaN if either head is NaN (fminf alone would drop it)
+    const float next_q = (isnan(a) || isnan(b)) ? __int_as_float(0x7fffffff) : fminf(a, b);
     const float entropy_term = __fmul_rn(alpha, log_prob[i]);        // temperature * log_prob
     const float soft = __fsub_rn(next_q, entropy_term);              // next_q - entropy_term
     const float w = __fmul_rn(discount[i], __fsub_rn(1.0f, terminal[i])); // discount * (1 - term)
@@ -67,6 +69,11 @@ extern "C" int b2rl_polyak(const b2rl_tensor_pair *pairs_host, int32_t n_pairs, 
     B2RL_REQUIRE(pairs_host || n_pairs == 0, B2RL_ERR_INVALID, "polyak: null pairs");
     B2RL_REQUIRE(n_pairs >= 0, B2RL_ERR_RANGE, "polyak: negative count");
     B2RL_REQUIRE(tau >= 0.0 && tau <= 1.0, B2RL_ERR_RANGE, "polyak: tau must be in [0, 1]");
+    // every pair is checked before the first launch, so a refused call changes no target
+    for (int i = 0; i < n_pairs; i++) {
+        const b2rl_tensor_pair &p = pairs_host[i];
+        B2RL_REQUIRE(p.dst && p.src && p.numel >= 0, B2RL_ERR_INVALID, "polyak: bad pair %d", i);
+    }
     cudaStream_t s = (cudaStream_t)stream;
     for (int done = 0; done < n_pairs; done += POLYAK_MAX) {
         PolyakArgs a;
@@ -76,8 +83,6 @@ extern "C" int b2rl_polyak(const b2rl_tensor_pair *pairs_host, int32_t n_pairs, 
         int blocks = 0;
         for (int i = 0; i < a.n; i++) {
             const b2rl_tensor_pair &p = pairs_host[done + i];
-            B2RL_REQUIRE(p.dst && p.src && p.numel >= 0, B2RL_ERR_INVALID, "polyak: bad pair %d",
-                         done + i);
             a.dst[i] = (float *)p.dst;
             a.src[i] = (const float *)p.src;
             a.numel[i] = p.numel;

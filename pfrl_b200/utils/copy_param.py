@@ -1,4 +1,6 @@
 """Parameter copies between networks (pfrl/utils/copy_param.py)."""
+import bisect
+
 import torch
 
 
@@ -7,34 +9,74 @@ def copy_param(target_link, source_link):
     target_link.load_state_dict(source_link.state_dict())
 
 
+_AVERAGED = (torch.float32, torch.float64, torch.float16)
+
+
+def _span(t):
+    return t.data_ptr(), t.data_ptr() + t.numel() * t.element_size()
+
+
+def _one_launch_ok(targets, sources):
+    """True when the pairs can go to b2rl_polyak together: all fp32, contiguous,
+    on one CUDA device, and no target shares memory with another target or with
+    a source (the kernel updates every pair at once, so a shared word would be
+    read and written by two CTAs)."""
+    device = targets[0].device
+    if device.type != "cuda":
+        return False
+    for t in targets + sources:
+        if t.device != device or t.dtype != torch.float32 or not t.is_contiguous():
+            return False
+    spans = sorted(_span(t) for t in targets)
+    for (_, end), (begin, _) in zip(spans, spans[1:]):
+        if begin < end:
+            return False
+    begins = [b for b, _ in spans]
+    for s in sources:
+        s_begin, s_end = _span(s)
+        # the last target that starts before the source ends is the only one that
+        # can overlap it (targets are disjoint and sorted)
+        i = bisect.bisect_left(begins, s_end) - 1
+        if i >= 0 and spans[i][1] > s_begin:
+            return False
+    return True
+
+
 @torch.no_grad()
 def soft_copy_param(target_link, source_link, tau):
-    """Polyak averaging ``target = (1 - tau) * target + tau * source`` over
-    floating state_dict entries; integer buffers are copied
-    (copy_param.py:9-22).  One launch for all tensors on CUDA (b2rl_polyak)."""
+    """Polyak averaging ``target = (1 - tau) * target + tau * source`` over the
+    fp32, fp64 and fp16 state_dict entries, in state_dict order
+    (copy_param.py:9-22).  Every other entry (integer buffers such as
+    BatchNorm's ``num_batches_tracked``, bf16 tensors) is left as it is: the
+    reference rebinds them in a copy of the target's state_dict, which does not
+    touch the target module.
+
+    When every averaged pair is fp32, contiguous, on one CUDA device and no
+    target shares memory with another target or a source, all pairs go in one
+    launch (b2rl_polyak), rounded like the reference.  Otherwise the
+    reference's own per-entry loop runs, so other dtypes round as it does and a
+    tied parameter (one tensor under two names) is averaged twice."""
     tgt = target_link.state_dict()
     src = source_link.state_dict()
     f_t, f_s = [], []
     for k, tv in tgt.items():
         sv = src[k]
-        if tv.dtype in (torch.float16, torch.bfloat16, torch.float32, torch.float64):
+        if sv.dtype in _AVERAGED:
             assert tv.shape == sv.shape
-            f_t.append(tv)
-            f_s.append(sv)
-        else:
-            tv.copy_(sv)
+            if tv.numel():
+                f_t.append(tv)
+                f_s.append(sv)
     if not f_t:
         return
-    if all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and s.is_cuda
-           and s.dtype == torch.float32 and s.is_contiguous() for t, s in zip(f_t, f_s)):
-        # one launch for the whole network (csrc/sac.cu, K9), rounded like the
-        # reference's target.mul_(1 - tau); target.add_(tau * source)
+    if _one_launch_ok(f_t, f_s):
+        # one launch for the whole network (csrc/sac.cu, K9)
         from pfrl_b200.ops.sac import polyak_
 
         polyak_(f_t, f_s, tau)
     else:
-        torch._foreach_mul_(f_t, 1.0 - tau)
-        torch._foreach_add_(f_t, f_s, alpha=tau)
+        for tv, sv in zip(f_t, f_s):
+            tv.mul_(1 - tau)
+            tv.add_(tau * sv)
 
 
 def copy_grad(target_link, source_link):
