@@ -503,6 +503,58 @@ int b2rl_ppo_loss(const float *log_prob, const float *entropy,
                   float *g_v_pred, double *scratch, float *losses, void *stream);
 
 /* ------------------------------------------------------------------------
+ * TRPO policy update (pfrl/agents/trpo.py:415-699, pfrl/utils/
+ * conjugate_gradient.py): fp32 storage, fp64 accumulation, device pointers.
+ * kind 0 = Independent(Normal(loc, scale), 1): params loc, scale [N, A] and
+ * actions fp32 [N, A]; kind 1 = Categorical(logits): params logits [N, K]
+ * (A = K, p1 / old1 / g1 / u1 / m1 unused) and actions int64 [N].
+ * ---------------------------------------------------------------------- */
+
+/* gain = mean(exp(logp - log_prob_old) * adv) + entropy_coef * mean(entropy),
+ * kl = mean KL(old || new), by torch's formulas (Normal log_prob / entropy /
+ * kl, Categorical's normalised logits, p_old == 0 -> 0 and p_new == 0 -> inf).
+ * adv_stats = {mean, std} standardises adv as (adv - mean) / (std + 1e-8) in
+ * fp32, or NULL.  out[3] = gain, kl, mean entropy.  g0 (and g1) non-NULL also
+ * write d gain / d params per row.  scratch: 3 doubles per 256 rows. */
+int b2rl_trpo_objective(int32_t kind, int32_t N, int32_t A, const float *p0,
+                        const float *p1, const float *old0, const float *old1,
+                        const void *actions, const float *log_prob_old,
+                        const float *adv, const float *adv_stats,
+                        double entropy_coef, float *g0, float *g1,
+                        double *scratch, float *out, void *stream);
+
+/* Fisher metric of the distribution parameters at p, applied to the tangent u
+ * and divided by N: diag(1/scale^2, 2/scale^2) (Gaussian; m1 may be NULL for a
+ * constant scale) or diag(p) - p p^T on the logits (categorical). */
+int b2rl_trpo_fisher(int32_t kind, int32_t N, int32_t A, const float *p0,
+                     const float *p1, const float *u0, const float *u1,
+                     float *m0, float *m1, void *stream);
+
+/* Conjugate gradient on n floats (one CTA per launch).  init: x = 0, r = p =
+ * b, state[2] doubles = {r.r, converged}.  iter (once per CG iteration, with
+ * Ap = A p): alpha = rr / p.Ap, x += alpha p, r -= alpha Ap, then either
+ * ||r|| < tol marks the state converged (later iterations return at once) or
+ * p = r + (r.r / rr) p.  step: dId = float(x.Ax), full_step =
+ * float(sqrt(2 max_kl / (dId + 1e-8))) * x; dId may be NULL. */
+int b2rl_trpo_cg_init(int64_t n, const float *b, float *x, float *r, float *p,
+                      double *state, void *stream);
+int b2rl_trpo_cg_iter(int64_t n, const float *Ap, float *x, float *r, float *p,
+                      double *state, double tol, void *stream);
+int b2rl_trpo_cg_step(int64_t n, const float *x, const float *Ax, double max_kl,
+                      float *full_step, float *dId, void *stream);
+
+/* Line-search decision over n_cand (<= 64) evaluated candidates theta_old +
+ * 2^-i full_step: cand[i][3] and gain0[3] are objective outputs.  The first
+ * candidate with a finite gain and KL, double(gain_i) - double(gain0) >= 0 and
+ * kl_i <= max_kl wins.  theta = theta_old + 2^-i * full_step (fp32 multiply,
+ * then add), or theta_old bit for bit when none wins.  record[3] = winner's
+ * kl, its step size (0 if none), 1 if one won. */
+int b2rl_trpo_line_search(int32_t n_cand, const float *cand, const float *gain0,
+                          double max_kl, int64_t n, const float *theta_old,
+                          const float *full_step, float *theta, float *record,
+                          void *stream);
+
+/* ------------------------------------------------------------------------
  * SAC / TD3 / DDPG update tail (fp32, device pointers).
  * ---------------------------------------------------------------------- */
 

@@ -256,7 +256,104 @@ def _compute_explained_variance(transitions):
     return float(1 - np.var(teacher - pred) / var)
 
 
-class PPO(agent.AttributeSavingMixin, agent.BatchAgent):
+class _DeviceRollout:
+    """The non-recurrent device rollout shared by PPO and TRPO: per vector step the raw
+    states, actions, next states, rewards, nonterminal and episode-cut flags, the finished
+    episodes in completion order, and the dataset pass (two forwards of ``self.model``,
+    the fused GAE).  The agent provides ``model``, ``obs_normalizer``, ``gamma``,
+    ``lambd``, ``use_fused`` and ``device``."""
+
+    def _rollout_clear(self, E=None):
+        self._states, self._next_states, self._actions = [], [], []
+        self._rewards, self._nonterminal, self._cut = [], [], []
+        self._segments = []     # finished episodes: (env, t_start, t_end) in completion order
+        self._seg_start = None if E is None else [0] * E  # per env: first step of its episode
+
+    def _record_act(self, raw, action, num_envs):
+        self._cur_state = raw
+        self._cur_action = action
+        if self._seg_start is None:
+            self._seg_start = [0] * num_envs
+
+    def _record_observe(self, batch_obs, batch_reward, batch_done, batch_reset):
+        """Append the step acted on last; returns the number of steps in the rollout."""
+        assert self._cur_state is not None
+        next_raw = self.batch_states(batch_obs, self.device, self.phi)
+        done = np.asarray(batch_done, dtype=bool)
+        end = np.logical_or(done, np.asarray(batch_reset, dtype=bool))
+        t = len(self._rewards)
+        self._states.append(self._cur_state)
+        self._actions.append(self._cur_action)
+        self._next_states.append(next_raw)
+        self._rewards.append(np.asarray(batch_reward, dtype=np.float32))
+        self._nonterminal.append((~done).astype(np.float32))
+        self._cut.append(end.astype(np.uint8))
+        for i in np.nonzero(end)[0]:  # episode completion order = env order within a step
+            self._segments.append((int(i), self._seg_start[i], t))
+            self._seg_start[i] = t + 1
+        self._cur_state = None
+        self._cur_action = None
+        return t + 1
+
+    def _dataset_order(self, T, E):
+        """Flat indices t*E + e in the order of the reference's dataset list:
+        finished episodes in completion order, then (flush, ppo.py:450-458)
+        the unfinished ones by env index."""
+        segs = list(self._segments)
+        for e in range(E):
+            if self._seg_start[e] <= T - 1:
+                segs.append((e, self._seg_start[e], T - 1))
+        order = list(itertools.chain.from_iterable(
+            (range(s * E + e, (t_end + 1) * E + e, E)) for e, s, t_end in segs))
+        assert len(order) == T * E
+        return order
+
+    def _rollout_dataset(self):
+        """_make_dataset (ppo.py:110-142, :36-53) on the rollout: flat [T*E] states,
+        actions, log pi_old, V, advantages, V targets, the advantage moments [2] = mean,
+        std (unbiased=False), and the reference's dataset order."""
+        T, dev = len(self._rewards), self.device
+        states = torch.stack(self._states)            # [T, E, ...]
+        next_states = torch.stack(self._next_states)
+        actions = torch.stack(self._actions)
+        E = states.shape[1]
+        N = T * E
+        reward = torch.as_tensor(np.stack(self._rewards), device=dev)
+        nonterminal = torch.as_tensor(np.stack(self._nonterminal), device=dev)
+        cut_np = np.stack(self._cut)
+        cut_np[T - 1, :] = 1  # flush of unfinished episodes
+        cut = torch.as_tensor(cut_np, device=dev)
+        order = self._dataset_order(T, E)
+
+        flat_s = states.reshape((N,) + states.shape[2:])
+        flat_ns = next_states.reshape((N,) + states.shape[2:])
+        flat_a = actions.reshape((N,) + actions.shape[2:])
+        norm = self.obs_normalizer
+        with torch.no_grad(), evaluating(self.model):
+            distribs, vs_pred = self.model(norm(flat_s, update=False) if norm else flat_s)
+            _, next_vs_pred = self.model(norm(flat_ns, update=False) if norm else flat_ns)
+            log_probs_old = distribs.log_prob(flat_a).float()
+            v = vs_pred.reshape(T, E).float()
+            v_next = next_vs_pred.reshape(T, E).float()
+        if self.use_fused and dev.type == "cuda":
+            adv, v_teacher, stats = fused.gae(reward, nonterminal, v, v_next, cut, self.gamma,
+                                              self.lambd)
+        else:
+            adv, v_teacher = _gae_torch(reward, nonterminal, v, v_next, cut, self.gamma, self.lambd)
+            std, mean = torch.std_mean(adv, unbiased=False)
+            stats = torch.stack([mean, std])
+        return dict(flat_s=flat_s, flat_a=flat_a, log_probs_old=log_probs_old, v_old=v.reshape(N),
+                    adv=adv, v_teacher=v_teacher, stats=stats, order=order, E=E, N=N)
+
+    def _explained_variance_from(self, v_teacher, v_old):
+        """ppo.py:56-62 on the device; read lazily by get_statistics."""
+        var_t = torch.var(v_teacher, unbiased=False)
+        ev = 1 - torch.var(v_teacher - v_old, unbiased=False) / var_t
+        self._explained_variance_t = torch.where(var_t == 0, torch.full_like(ev, float("nan")), ev)
+        self.explained_variance = None
+
+
+class PPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
     saved_attributes = ("model", "optimizer", "obs_normalizer")
 
     def __init__(self, model, optimizer, obs_normalizer=None, gpu=None, gamma=0.99, lambd=0.95,
@@ -315,10 +412,7 @@ class PPO(agent.AttributeSavingMixin, agent.BatchAgent):
                 if "capturable" in group:
                     group["capturable"] = True
         # rollout (device tensors per vector step)
-        self._states, self._next_states, self._actions = [], [], []
-        self._rewards, self._nonterminal, self._cut = [], [], []
-        self._segments = []     # finished episodes: (env, t_start, t_end) in completion order
-        self._seg_start = None  # per env: first step of the running episode
+        self._rollout_clear()
         self._cur_state = None
         self._cur_action = None
         # recurrent: batched states on the device, and per vector step the flattened
@@ -358,10 +452,7 @@ class PPO(agent.AttributeSavingMixin, agent.BatchAgent):
             action = action_distrib.sample()
             self.entropy_record.extend(action_distrib.entropy())
             self.value_record.extend(batch_value)
-        self._cur_state = raw
-        self._cur_action = action
-        if self._seg_start is None:
-            self._seg_start = [0] * len(batch_obs)
+        self._record_act(raw, action, len(batch_obs))
         return action.cpu().numpy()
 
     def _recurrent_step(self, feat):
@@ -396,23 +487,8 @@ class PPO(agent.AttributeSavingMixin, agent.BatchAgent):
                 self.test_recurrent_states = self._mask_ended(
                     self.test_recurrent_states, batch_done, batch_reset)
             return
-        assert self._cur_state is not None
         num_envs = len(batch_obs)
-        next_raw = self.batch_states(batch_obs, self.device, self.phi)
-        done = np.asarray(batch_done, dtype=bool)
-        end = np.logical_or(done, np.asarray(batch_reset, dtype=bool))
-        t = len(self._rewards)
-        self._states.append(self._cur_state)
-        self._actions.append(self._cur_action)
-        self._next_states.append(next_raw)
-        self._rewards.append(np.asarray(batch_reward, dtype=np.float32))
-        self._nonterminal.append((~done).astype(np.float32))
-        self._cut.append(end.astype(np.uint8))
-        for i in np.nonzero(end)[0]:  # episode completion order = env order within a step
-            self._segments.append((int(i), self._seg_start[i], t))
-            self._seg_start[i] = t + 1
-        self._cur_state = None
-        self._cur_action = None
+        steps = self._record_observe(batch_obs, batch_reward, batch_done, batch_reset)
         if self.recurrent:
             rows, present = self._cur_rs
             self._rstates.append(rows)
@@ -420,63 +496,24 @@ class PPO(agent.AttributeSavingMixin, agent.BatchAgent):
             self._cur_rs = None
             self.train_recurrent_states = self._mask_ended(
                 self.train_recurrent_states, batch_done, batch_reset)
-        if (t + 1) * num_envs >= self.update_interval:
+        if steps * num_envs >= self.update_interval:
             if self.recurrent:
                 self._update_recurrent_from_rollout()
             else:
                 self._update_from_rollout()
 
     # ------------------------------------------------------------ the update
-    def _dataset_order(self, T, E):
-        """Flat indices t*E + e in the order of the reference's dataset list:
-        finished episodes in completion order, then (flush, ppo.py:450-458)
-        the unfinished ones by env index."""
-        segs = list(self._segments)
-        for e in range(E):
-            if self._seg_start[e] <= T - 1:
-                segs.append((e, self._seg_start[e], T - 1))
-        order = list(itertools.chain.from_iterable(
-            (range(s * E + e, (t_end + 1) * E + e, E)) for e, s, t_end in segs))
-        assert len(order) == T * E
-        return order
-
     def _update_from_rollout(self):
-        T, dev = len(self._rewards), self.device
-        states = torch.stack(self._states)            # [T, E, ...]
-        next_states = torch.stack(self._next_states)
-        actions = torch.stack(self._actions)
-        E = states.shape[1]
-        N = T * E
-        reward = torch.as_tensor(np.stack(self._rewards), device=dev)
-        nonterminal = torch.as_tensor(np.stack(self._nonterminal), device=dev)
-        cut_np = np.stack(self._cut)
-        cut_np[T - 1, :] = 1  # flush of unfinished episodes
-        cut = torch.as_tensor(cut_np, device=dev)
-        order = self._dataset_order(T, E)
-
-        flat_s = states.reshape((N,) + states.shape[2:])
-        flat_ns = next_states.reshape((N,) + states.shape[2:])
-        flat_a = actions.reshape((N,) + actions.shape[2:])
-        norm = self.obs_normalizer
-        # _add_log_prob_and_value_to_episodes (ppo.py:110-142)
-        with torch.no_grad(), evaluating(self.model):
-            distribs, vs_pred = self.model(norm(flat_s, update=False) if norm else flat_s)
-            _, next_vs_pred = self.model(norm(flat_ns, update=False) if norm else flat_ns)
-            log_probs_old = distribs.log_prob(flat_a).float()
-            v = vs_pred.reshape(T, E).float()
-            v_next = next_vs_pred.reshape(T, E).float()
-        # GAE (ppo.py:36-53) + advantage moments (:476-478)
-        if self.use_fused and dev.type == "cuda":
-            adv, v_teacher, stats = fused.gae(reward, nonterminal, v, v_next, cut, self.gamma,
-                                              self.lambd)
-        else:
-            adv, v_teacher = _gae_torch(reward, nonterminal, v, v_next, cut, self.gamma, self.lambd)
-            std, mean = torch.std_mean(adv, unbiased=False)
-            stats = torch.stack([mean, std])
+        dev = self.device
+        d = self._rollout_dataset()
+        flat_s, flat_a, log_probs_old = d["flat_s"], d["flat_a"], d["log_probs_old"]
+        adv, v_teacher, stats, order, E, N = (d["adv"], d["v_teacher"], d["stats"], d["order"],
+                                              d["E"], d["N"])
         if self.stats_sync is not None and self.standardize_advantages:
             stats = self.stats_sync(adv)
         adv, v_teacher = adv.reshape(N), v_teacher.reshape(N)
-        v_old = v.reshape(N)
+        v_old = d["v_old"]
+        norm = self.obs_normalizer
 
         if norm:  # _update_obs_normalizer (ppo.py:460-463), after the dataset is built
             norm.experience(flat_s)
@@ -494,15 +531,8 @@ class PPO(agent.AttributeSavingMixin, agent.BatchAgent):
                                      adv_stats)
                 self.n_updates += 1
 
-        # explained variance of the value predictions (ppo.py:56-62)
-        var_t = torch.var(v_teacher, unbiased=False)
-        ev = 1 - torch.var(v_teacher - v_old, unbiased=False) / var_t
-        self._explained_variance_t = torch.where(var_t == 0, torch.full_like(ev, float("nan")), ev)
-        self.explained_variance = None
-        self._states, self._next_states, self._actions = [], [], []
-        self._rewards, self._nonterminal, self._cut = [], [], []
-        self._segments = []
-        self._seg_start = [0] * E
+        self._explained_variance_from(v_teacher, v_old)
+        self._rollout_clear(E)
 
     # -------------------------------------------------------- recurrent update
     def _episode_spans(self, T, E):
@@ -611,15 +641,9 @@ class PPO(agent.AttributeSavingMixin, agent.BatchAgent):
                 self.optimizer.step()
                 self.n_updates += 1
 
-        var_t = torch.var(v_teacher, unbiased=False)
-        ev = 1 - torch.var(v_teacher - v_old, unbiased=False) / var_t
-        self._explained_variance_t = torch.where(var_t == 0, torch.full_like(ev, float("nan")), ev)
-        self.explained_variance = None
-        self._states, self._next_states, self._actions = [], [], []
-        self._rewards, self._nonterminal, self._cut = [], [], []
+        self._explained_variance_from(v_teacher, v_old)
+        self._rollout_clear(E)
         self._rstates, self._rpresent = [], []
-        self._segments = []
-        self._seg_start = [0] * E
 
     def _minibatch_step(self, s, a, log_probs_old, v_old, advs, v_teacher, adv_stats,
                         record=True):

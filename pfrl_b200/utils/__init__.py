@@ -1,5 +1,6 @@
 from pfrl_b200.utils.batch_states import batch_states  # NOQA
 from pfrl_b200.utils.clip_l2_grad_norm import clip_l2_grad_norm_  # NOQA
+from pfrl_b200.utils.conjugate_gradient import conjugate_gradient  # NOQA
 from pfrl_b200.utils.modes import evaluating  # NOQA
 from pfrl_b200.utils.copy_param import synchronize_parameters  # NOQA
 from pfrl_b200.utils.random import sample_n_k  # NOQA

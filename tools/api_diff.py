@@ -46,7 +46,7 @@ action_value.SingleActionValue
 METHOD_CLASSES = """
 agents.DQN agents.CategoricalDoubleDQN agents.IQN agents.PPO agents.A2C agents.SoftActorCritic
 agents.AL agents.PAL agents.DoublePAL agents.DPP agents.dpp.DPPL agents.dpp.DPPGreedy
-agents.TD3 agents.DDPG replay_buffers.ReplayBuffer replay_buffers.PrioritizedReplayBuffer
+agents.TD3 agents.DDPG agents.TRPO replay_buffers.ReplayBuffer replay_buffers.PrioritizedReplayBuffer
 replay_buffer.ReplayUpdater replay_buffers.EpisodicReplayBuffer nn.EmpiricalNormalization nn.FactorizedNoisyLinear
 envs.MultiprocessVectorEnv envs.SerialVectorEnv wrappers.VectorFrameStack
 action_value.DiscreteActionValue action_value.DistributionalDiscreteActionValue
