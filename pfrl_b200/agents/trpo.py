@@ -8,7 +8,7 @@ The rollout, its episode segmentation, the dataset order and the dataset pass
 value function is trained on fixed-size minibatches of PPO's index stream.
 
 The policy update is the reference's full-batch pass (trpo.py:415-699).  With
-a Gaussian (``Independent(Normal)``) or categorical policy on CUDA it runs
+an fp32 Gaussian (``Independent(Normal)``) or categorical policy on CUDA it runs
 without a device-to-host copy or synchronisation (csrc/trpo.cu):
   * one forward, and the objective kernel for the gain and d gain / d(dist
     params), back-propagated once to the parameters;
@@ -25,7 +25,8 @@ copy of the candidates' values, and only when the logger takes INFO.  With ``cud
 fused policy update and the value-function minibatch step are each replayed as one
 CUDA graph.
 
-Everything else (CPU, ``use_fused = False``, other distributions) runs the
+Everything else (CPU, ``use_fused = False``, other distributions, fp64 or half
+policies) runs the
 reference's algorithm in the reference's operation order.
 """
 from logging import INFO, getLogger
@@ -91,6 +92,10 @@ def _distribution_params(distrib):
     if type(distrib) is D.Categorical and distrib.logits.dim() == 2:
         return fused.CATEGORICAL, [distrib.logits]
     return None
+
+
+def _fp32_on(device, tensors):
+    return all(t.dtype == torch.float32 and t.device == device for t in tensors)
 
 
 class _RecordRing(_DeviceRing):
@@ -258,16 +263,21 @@ class TRPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
         # the policy's full batch in dataset order (trpo.py:432-451)
         s, a = obs[idx], d["flat_a"][idx]
         lp_old, adv_b = d["log_probs_old"][idx], adv[idx]
-        self._line_search_log = None
-        stats = d["stats"] if self.standardize_advantages else None
-        if not (self.use_fused and self.device.type == "cuda"
-                and self._update_policy_fused(s, a, lp_old, adv_b, stats)):
-            self._update_policy_torch(s, a, lp_old, self._standardized(adv_b))
+        self._update_policy(s, a, lp_old, adv_b,
+                            d["stats"] if self.standardize_advantages else None)
         self._update_vf(obs, v_teacher, order)
         self._explained_variance_from(v_teacher, d["v_old"])
         self._rollout_clear(E)
         if self._line_search_log is not None and self.logger.isEnabledFor(INFO):
             self._log_line_search(*self._line_search_log)
+
+    def _update_policy(self, states, actions, log_prob_old, advs, adv_stats):
+        """The fused update where it applies, else the reference's formulation.
+        ``adv_stats`` (mean, std of ``advs``) is given when advantages are standardised."""
+        self._line_search_log = None
+        if not (self.use_fused and self.device.type == "cuda"
+                and self._update_policy_fused(states, actions, log_prob_old, advs, adv_stats)):
+            self._update_policy_torch(states, actions, log_prob_old, self._standardized(advs))
 
     def _standardized(self, advs):
         if not self.standardize_advantages:
@@ -413,12 +423,18 @@ class TRPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
 
     # ------------------------------------------------------ the fused update
     def _fused_kind(self, states):
-        """The kernels' kind of the policy's distribution, or False for one they do not
-        cover; found once, on a one-row forward."""
+        """The kernels' kind of the policy's distribution, or False where they do not apply:
+        a distribution they do not cover, or a policy whose parameters or distribution
+        parameters are not all fp32 on the agent's device (the kernels are fp32; an fp64 or
+        half policy takes the reference's formulation).  The distribution is classified
+        once, on a one-row forward; the parameters are checked on every call."""
+        if not _fp32_on(self.device, self.policy.parameters()):
+            return False
         if self._policy_kind is None:
             with torch.no_grad(), evaluating(self.policy), no_distribution_validation():
                 kind_params = _distribution_params(self.policy(states[:1]))
-            self._policy_kind = False if kind_params is None else kind_params[0]
+            covered = kind_params is not None and _fp32_on(self.device, kind_params[1])
+            self._policy_kind = kind_params[0] if covered else False
         return self._policy_kind
 
     def _update_policy_fused(self, states, actions, log_prob_old, advs, adv_stats):

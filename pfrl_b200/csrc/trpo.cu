@@ -65,6 +65,12 @@ __device__ double row_lse(const float *z, int K)
     return m + log(s);
 }
 
+// Whether a category's probability counts as nonzero.  torch decides p == 0 on the fp32
+// probabilities of a float32 Categorical (the KL's inf and 0 terms, the entropy's clamped
+// logits), so the test is on the fp32 rounding of p; the value used is still the fp64 one.
+// p = e^l rounds to 0 below l = -103.97 (half the smallest subnormal).
+__device__ __forceinline__ bool prob_nonzero(double p) { return (float)p != 0.0f; }
+
 __global__ void __launch_bounds__(256) k_trpo_objective(ObjArgs a)
 {
     __shared__ double sh[3][8];
@@ -98,9 +104,9 @@ __global__ void __launch_bounds__(256) k_trpo_objective(ObjArgs a)
                 const double l = (double)z[k] - lse, lo = (double)zo[k] - lse_o;
                 const double p = exp(l), po = exp(lo);
                 // Categorical.entropy clamps the logits at finfo.min: p = 0 adds nothing
-                if (p > 0.0) ent -= p * l;
+                if (prob_nonzero(p)) ent -= p * l;
                 // _kl_categorical_categorical: p_old = 0 -> 0, else q = 0 -> inf
-                if (po > 0.0) kl += p > 0.0 ? po * (lo - l) : INFINITY;
+                if (prob_nonzero(po)) kl += prob_nonzero(p) ? po * (lo - l) : INFINITY;
             }
         }
         const double ratio = exp(lp - (double)a.log_prob_old[i]);
@@ -121,12 +127,12 @@ __global__ void __launch_bounds__(256) k_trpo_objective(ObjArgs a)
                 double h = 0.0;
                 for (int k = 0; k < a.A; k++) {
                     const double l = (double)z[k] - lse, p = exp(l);
-                    if (p > 0.0) h -= p * l;
+                    if (prob_nonzero(p)) h -= p * l;
                 }
                 // d logp(a)/dz_k = [k == a] - p_k;  dH/dz_k = -p_k (log p_k + H)
                 for (int k = 0; k < a.A; k++) {
                     const double l = (double)z[k] - lse, p = exp(l);
-                    const double dh = p > 0.0 ? -p * (l + h) : 0.0;
+                    const double dh = prob_nonzero(p) ? -p * (l + h) : 0.0;
                     a.g0[row + k] = (float)(ra * ((k == act ? 1.0 : 0.0) - p) + c * dh);
                 }
             }

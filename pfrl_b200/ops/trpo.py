@@ -10,8 +10,22 @@ from pfrl_b200.ops.ppo import _f32, _p, _stream
 GAUSSIAN, CATEGORICAL = 0, 1
 
 
+def _cuda(t):
+    """``t`` as an fp32 contiguous CUDA tensor (a copy if it is not one already)."""
+    assert t.is_cuda, "the TRPO kernels take CUDA tensors"
+    return _f32(t)
+
+
+def _buffer(t, name):
+    """A tensor a kernel writes in place: it must already be fp32, contiguous and on CUDA,
+    since a converted copy would take the write."""
+    assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous(), \
+        "%s must be a contiguous fp32 CUDA tensor, got %s %s" % (name, t.dtype, t.device)
+    return t
+
+
 def _rows(t, N):
-    return _f32(t).reshape(N, -1)
+    return _cuda(t).reshape(N, -1)
 
 
 def _actions(kind, actions, N):
@@ -35,8 +49,8 @@ def _objective(kind, params, old, actions, log_prob_old, adv, adv_stats, entropy
     g1 = g[1] if kind == GAUSSIAN else None
     _lib.check(L.b2rl_trpo_objective(
         kind, N, A, _p(p[0]), _p(p1), _p(o[0]), _p(o1), _p(_actions(kind, actions, N)),
-        _p(_f32(log_prob_old).view(-1)), _p(_f32(adv).view(-1)),
-        _p(None if adv_stats is None else _f32(adv_stats)), float(entropy_coef), _p(g[0]),
+        _p(_cuda(log_prob_old).view(-1)), _p(_cuda(adv).view(-1)),
+        _p(None if adv_stats is None else _cuda(adv_stats)), float(entropy_coef), _p(g[0]),
         _p(g1), _p(scratch), _p(out), _stream()))
     return out, g
 
@@ -89,7 +103,7 @@ def fisher(kind, params, tangents):
 def cg_init(b):
     """x = 0, r = p = b; returns (x, r, p, state) for cg_iter."""
     L = _lib.load()
-    b = _f32(b).view(-1)
+    b = _cuda(b).view(-1)
     x, r, p = torch.empty_like(b), torch.empty_like(b), torch.empty_like(b)
     state = torch.empty(2, dtype=torch.float64, device=b.device)
     _lib.check(L.b2rl_trpo_cg_init(b.numel(), _p(b), _p(x), _p(r), _p(p), _p(state), _stream()))
@@ -98,17 +112,25 @@ def cg_init(b):
 
 def cg_iter(Ap, x, r, p, state, tol):
     L = _lib.load()
-    _lib.check(L.b2rl_trpo_cg_iter(x.numel(), _p(_f32(Ap).view(-1)), _p(x), _p(r), _p(p),
-                                   _p(state), float(tol), _stream()))
+    for t, name in ((x, "x"), (r, "r"), (p, "p")):
+        _buffer(t, name)
+    assert state.is_cuda and state.dtype == torch.float64 and state.numel() == 2
+    Ap = _cuda(Ap).view(-1)
+    assert Ap.numel() == x.numel() == r.numel() == p.numel()
+    _lib.check(L.b2rl_trpo_cg_iter(x.numel(), _p(Ap), _p(x), _p(r), _p(p), _p(state),
+                                   float(tol), _stream()))
 
 
 def cg_step(x, Ax, max_kl):
     """Returns (full_step = sqrt(2 max_kl / (dId + 1e-8)) * x, dId [1])."""
     L = _lib.load()
+    x = _cuda(x).view(-1)
+    Ax = _cuda(Ax).view(-1)
+    assert Ax.numel() == x.numel()
     full = torch.empty_like(x)
     dId = torch.empty(1, dtype=torch.float32, device=x.device)
-    _lib.check(L.b2rl_trpo_cg_step(x.numel(), _p(x), _p(_f32(Ax).view(-1)), float(max_kl),
-                                   _p(full), _p(dId), _stream()))
+    _lib.check(L.b2rl_trpo_cg_step(x.numel(), _p(x), _p(Ax), float(max_kl), _p(full), _p(dId),
+                                   _stream()))
     return full, dId
 
 
@@ -116,12 +138,15 @@ def line_search(cand, gain0, max_kl, theta_old, full_step, theta=None):
     """cand [C, 3], gain0 [3]: objective outputs.  Writes theta (new or given) and returns
     (theta, record[3] = accepted KL, step size (0 if none), 1 if accepted)."""
     L = _lib.load()
-    cand = _f32(cand)
-    theta_old, full_step = _f32(theta_old).view(-1), _f32(full_step).view(-1)
+    cand, gain0 = _cuda(cand), _cuda(gain0)
+    theta_old, full_step = _cuda(theta_old).view(-1), _cuda(full_step).view(-1)
+    assert cand.dim() == 2 and cand.shape[1] == 3 and gain0.numel() >= 1
+    assert full_step.numel() == theta_old.numel()
     if theta is None:
         theta = torch.empty_like(theta_old)
+    assert _buffer(theta, "theta").numel() == theta_old.numel()
     record = torch.empty(3, dtype=torch.float32, device=theta.device)
-    _lib.check(L.b2rl_trpo_line_search(cand.shape[0], _p(cand), _p(_f32(gain0)), float(max_kl),
+    _lib.check(L.b2rl_trpo_line_search(cand.shape[0], _p(cand), _p(gain0), float(max_kl),
                                        theta_old.numel(), _p(theta_old), _p(full_step),
                                        _p(theta), _p(record), _stream()))
     return theta, record

@@ -76,6 +76,49 @@ def test_recurrent_trpo_is_refused():
         pfrl_b200.agents.TRPO(nn.Linear(2, 2), nn.Linear(2, 1), None, recurrent=True)
 
 
+@pytest.mark.parametrize("head", ["gauss", "softmax"])
+def test_fused_path_refuses_policies_that_are_not_fp32(head):
+    """The kernels read fp32: the fused update is taken only when every policy parameter
+    and every distribution parameter is fp32 on the agent's device."""
+    from torch import nn
+
+    import pfrl_b200
+    from pfrl_b200.ops import trpo as fused
+    from pfrl_b200.policies import (GaussianHeadWithStateIndependentCovariance,
+                                    SoftmaxCategoricalHead)
+
+    def agent_for(policy):
+        return pfrl_b200.agents.TRPO(policy, nn.Linear(3, 1), None)
+
+    def make(dtype=torch.float32):
+        h = GaussianHeadWithStateIndependentCovariance(2, var_type="diagonal") \
+            if head == "gauss" else SoftmaxCategoricalHead()
+        return nn.Sequential(nn.Linear(3, 2), h).to(dtype)
+
+    want = fused.GAUSSIAN if head == "gauss" else fused.CATEGORICAL
+    s = torch.randn(4, 3)
+    assert agent_for(make())._fused_kind(s) == want
+    for dtype in (torch.float64, torch.float16, torch.bfloat16):
+        assert agent_for(make(dtype))._fused_kind(s.to(dtype)) is False, dtype
+    # fp32 parameters, fp64 distribution parameters
+    cast = nn.Sequential(nn.Linear(3, 2), _Cast(torch.float64), make()[1])
+    assert agent_for(cast)._fused_kind(s) is False
+    # a policy converted after its first update is checked again
+    agent = agent_for(make())
+    assert agent._fused_kind(s) == want
+    agent.policy.double()
+    assert agent._fused_kind(s.double()) is False
+
+
+class _Cast(torch.nn.Module):
+    def __init__(self, dtype):
+        super().__init__()
+        self.dtype = dtype
+
+    def forward(self, x):
+        return x.to(self.dtype)
+
+
 def test_checkpoints_interchange_with_the_reference(tmp_path):
     from oracle import refimport
 

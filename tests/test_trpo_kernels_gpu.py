@@ -3,7 +3,12 @@
 Bounds: the kernels read fp32 inputs exactly, compute in fp64 and round each output
 to fp32 once, so an output differs from the fp64 value by at most one fp32 rounding
 (2^-24 relative) plus fp64 round-off; the bounds below are 4 fp32 ulps relative plus
-an absolute floor for values that cancel (KL near 0)."""
+an absolute floor for values that cancel (KL near 0).
+
+The categorical reference is evaluated in fp64 except for one decision: whether a
+probability is zero.  torch takes that from the fp32 probabilities of the fp32
+Categorical the policy returns (the KL's inf where q = 0 and 0 where p = 0, the entropy's
+clamped logits), so the restatement does too; e^l is 0 in fp32 below l = -103.97."""
 import numpy as np
 import pytest
 import torch
@@ -27,16 +32,54 @@ def ref_objective(kind, params, old, actions, lp_old, adv, stats, c):
         do = D.Independent(D.Normal(old[0].double(), old[1].double()), 1)
         lp = d.log_prob(actions.double())
     else:
-        d, do = D.Categorical(logits=p[0]), D.Categorical(logits=old[0].double())
+        d = D.Categorical(logits=p[0])
         lp = d.log_prob(actions)
-    ent = d.entropy()
+    if kind == fused.GAUSSIAN:
+        ent, kl = d.entropy(), D.kl_divergence(do, d)
+    else:
+        ent, kl = categorical_entropy_kl(p[0], old[0].double(), params[0], old[0])
     gain = torch.mean(torch.exp(lp - lp_old.double()) * adv.double()) + c * torch.mean(ent)
-    kl = torch.mean(D.kl_divergence(do, d))
+    kl = torch.mean(kl)
     grads = torch.autograd.grad(gain, p)
     return gain.detach(), kl.detach(), ent.mean().detach(), grads
 
 
-def make_case(kind, N, A, seed, extreme=False, zero_adv=False, neg_inf=False):
+def categorical_entropy_kl(z, zo, z32, zo32):
+    """Categorical.entropy and _kl_categorical_categorical(old, new) per row in fp64 (z, zo),
+    with p == 0 decided on the fp32 probabilities of the fp32 logits (z32, zo32)."""
+    nz = D.Categorical(logits=z32.float()).probs != 0
+    nzo = D.Categorical(logits=zo32.float()).probs != 0
+    l = z - torch.logsumexp(z, -1, keepdim=True)
+    lo = zo - torch.logsumexp(zo, -1, keepdim=True)
+    zero = torch.zeros((), dtype=torch.float64)
+    l_nz = torch.where(nz, l, zero)  # no -inf * 0 in the gradient of a masked term
+    ent = -torch.where(nz, l.exp() * l_nz, zero).sum(-1)
+    lo_nz = torch.where(nzo, lo, zero)
+    kl = torch.where(nzo, torch.where(nz, lo.exp() * (lo_nz - l_nz), float("inf")), zero)
+    return ent, kl.detach().sum(-1)
+
+
+def plant_underflow(z, zo, actions, rows=None):
+    """Rows whose normalised logits are 0 at the action, -80 elsewhere and -120 at one
+    other category: -120 only on the new side (torch: q = 0 in fp32, KL inf), only on the
+    old side (p = 0 in fp32, the term is 0), and on both.  -80 and -120 lie well inside
+    fp32's normal range and well below its smallest subnormal (e^-103.3)."""
+    K = z.shape[1]
+    rows = range(min(3, z.shape[0])) if rows is None else rows
+    for r in rows:
+        a = int(actions[r])
+        other = (a + 1) % K
+        for t in (z, zo):
+            t[r] = -80.0
+            t[r, a] = 0.0
+        if r % 3 in (0, 2):
+            z[r, other] = -120.0
+        if r % 3 in (1, 2):
+            zo[r, other] = -120.0
+
+
+def make_case(kind, N, A, seed, extreme=False, zero_adv=False, neg_inf=False,
+              underflow=False):
     g = torch.Generator().manual_seed(seed)
     if kind == fused.GAUSSIAN:
         loc = torch.randn(N, A, generator=g)
@@ -61,6 +104,8 @@ def make_case(kind, N, A, seed, extreme=False, zero_adv=False, neg_inf=False):
             zo[rows[1::3], other[1::3]] = -float("inf")
             z[rows[2::3], other[2::3]] = -float("inf")
             zo[rows[2::3], other[2::3]] = -float("inf")
+        if underflow:
+            plant_underflow(z, zo, actions, range(0, N, 7))
         params, old = [z], [zo]
         lp_old = D.Categorical(logits=zo.double()).log_prob(actions).float()
     adv = torch.zeros(N) if zero_adv else torch.randn(N, generator=g)
@@ -129,6 +174,60 @@ def test_categorical_zero_probabilities():
     out = fused.objective(fused.CATEGORICAL, [z.to(DEV)], [zo.to(DEV)], actions.to(DEV),
                           lp_old.to(DEV), adv.to(DEV), None, 0.01)
     assert torch.isfinite(out).all()
+
+
+@pytest.mark.parametrize("K", [3, 18])
+def test_categorical_underflow_is_decided_on_fp32_probabilities(K):
+    """A probability that is nonzero in fp64 but 0 in fp32 is 0, as torch decides it: KL
+    inf where the new side underflows, no term where the old side does."""
+    run_case(fused.CATEGORICAL, 301, K, seed=6, underflow=True)
+    params, old, actions, lp_old, adv = make_case(fused.CATEGORICAL, 30, K, 7)
+    z, zo = params[0], old[0]
+    plant_underflow(z, zo, actions)
+    lp_old = D.Categorical(logits=zo.double()).log_prob(actions).float()
+    dev = lambda t: t.to(DEV)  # noqa: E731
+    out = fused.objective(fused.CATEGORICAL, [dev(z)], [dev(zo)], dev(actions), dev(lp_old),
+                          dev(adv), None, 0.01).cpu()
+    # the reference's fp32 KL is inf; the fp64 rule alone would give e^-80 * 40 / 30
+    assert float(D.kl_divergence(D.Categorical(logits=zo), D.Categorical(logits=z)).mean()) \
+        == float("inf")
+    assert float(out[1]) == float("inf")
+    # without the new-side row: finite, and equal to the fp64 restatement
+    keep = list(range(1, 30))
+    zk, zok, ak, lpk, advk = (t[keep] for t in (z, zo, actions, lp_old, adv))
+    out = fused.objective(fused.CATEGORICAL, [dev(zk)], [dev(zok)], dev(ak), dev(lpk),
+                          dev(advk), None, 0.01).cpu().double()
+    want = ref_objective(fused.CATEGORICAL, [zk], [zok], ak, lpk, advk, None, 0.01)
+    assert np.isfinite(float(want[1]))
+    for got, w in zip(out, want[:3]):
+        assert abs(float(got) - float(w)) <= RT * abs(float(w)) + 1e-12, (float(got), float(w))
+
+
+def test_line_search_backtracks_from_a_kl_that_is_inf_in_fp32():
+    """Candidate 0 puts probability e^-120 (0 in fp32) where the old policy has e^-80: the
+    reference's KL is inf there and it backtracks to candidate 1 (theta_old, KL 0)."""
+    K, N = 5, 40
+    params, old, actions, _, _ = make_case(fused.CATEGORICAL, N, K, 8)
+    z, zo = params[0], old[0]
+    plant_underflow(z, zo, actions, rows=[0])
+    zo = z.clone()
+    zo[0, (int(actions[0]) + 1) % K] = -80.0
+    lp_old = D.Categorical(logits=zo.double()).log_prob(actions).float()
+    adv = torch.zeros(N)
+    dev = lambda t: t.to(DEV)  # noqa: E731
+    cand = torch.stack([
+        fused.objective(fused.CATEGORICAL, [dev(x)], [dev(zo)], dev(actions), dev(lp_old),
+                        dev(adv), None, 0.0) for x in (z, zo)])
+    gain0 = fused.objective(fused.CATEGORICAL, [dev(zo)], [dev(zo)], dev(actions), dev(lp_old),
+                            dev(adv), None, 0.0)
+    ref_kl = [float(D.kl_divergence(D.Categorical(logits=zo), D.Categorical(logits=x)).mean())
+              for x in (z, zo)]
+    assert ref_kl == [float("inf"), 0.0]
+    theta_old = torch.randn(50, device=DEV)
+    full = torch.randn(50, device=DEV)
+    theta, rec = fused.line_search(cand, gain0, 0.01, theta_old, full)
+    assert rec.cpu().tolist() == [0.0, 0.5, 1.0]
+    assert torch.equal(theta, theta_old + 0.5 * full)
 
 
 def _mlp_policy(kind, obs, A):
