@@ -30,6 +30,7 @@ import torch
 import torch.nn.functional as F
 
 from pfrl_b200 import _lib, agent
+from pfrl_b200.agents._graph import CapturedStep
 from pfrl_b200.ops import losses as fused
 from pfrl_b200.replay_buffer import (
     AbstractEpisodicReplayBuffer, ReplayUpdater, batch_experiences, batch_recurrent_experiences,
@@ -224,17 +225,14 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
         # update is launch-bound, e.g. Nature-DQN at batch 32).
         # With a grad_sync hook (data-parallel ranks) the update is TWO graphs around the
         # eagerly issued all-reduce: forward + loss + backward + bucket packing, then
-        # unpacking + clipping + optimizer step.
-        self._graph_enabled = bool(cuda_graph) and self.device.type == "cuda" \
-            and (grad_sync is None or all(hasattr(grad_sync, a) for a in ("pack", "reduce", "unpack")))
-        self._graph = None
-        self._graph_warmup = 0
-        self._act_graph = None
-        self._act_graph_warmup = 0
-        if self._graph_enabled:
-            for group in optimizer.param_groups:
-                if "capturable" in group:
-                    group["capturable"] = True
+        # unpacking + clipping + optimizer step.  The acting forward is a third graph.
+        self._graph = self._step_graph = self._act_graph = None
+        if cuda_graph and self.device.type == "cuda" and (grad_sync is None or all(
+                hasattr(grad_sync, a) for a in ("pack", "reduce", "unpack"))):
+            self._graph = CapturedStep(3, (optimizer,))
+            if grad_sync is not None:
+                self._step_graph = CapturedStep(3, share_pool_with=self._graph)
+            self._act_graph = CapturedStep(3)
         if (self.replay_buffer.capacity is not None
                 and self.replay_buffer.capacity < self.replay_updater.replay_start_size):
             raise ValueError("Replay start size cannot exceed replay buffer capacity.")
@@ -262,10 +260,10 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
                     dtype=torch.float32)
         want_list = errors_out is not None
         want_errors = has_weight or want_list
-        if self._graph_enabled:
-            loss, delta = self._learn_graphed(exp_batch, want_errors)
+        if self._graph is not None:
+            loss, delta, q = self._learn_graphed(exp_batch, want_errors)
         else:
-            loss, delta = self._learn(exp_batch, want_errors)
+            loss, delta, q = self._learn(exp_batch, want_errors)
         if want_list:
             del errors_out[:]
             errors_out.extend(delta.detach().cpu().numpy())
@@ -275,61 +273,52 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
             # reference calls update_errors between forward and backward,
             # dqn.py:356; the priorities only depend on the forward pass.)
             self.replay_buffer.update_errors(delta.detach())
-        self.loss_record.append(loss.detach())
-        self.q_record.extend(self._last_q)
+        self.loss_record.append(loss)
+        self.q_record.extend(q)
         self.optim_t += 1
 
     def _learn(self, exp_batch, want_errors):
         """loss -> backward -> (all-reduce) -> clip -> optimizer step; touches no
-        Python-side state, so it can be captured in a CUDA graph."""
+        Python-side state, so it can be captured in a CUDA graph.  Returns the loss,
+        |y - t| (or None) and the Q-values of the batch."""
+        out = self._backward(exp_batch, want_errors)
+        if self.grad_sync is not None:
+            self.grad_sync(self.model)
+        self._step()
+        return out
+
+    def _backward(self, exp_batch, want_errors):
         loss, delta = self._compute_loss(exp_batch, want_errors=want_errors)
         self.optimizer.zero_grad()
         loss.backward()
-        if self.grad_sync is not None:
-            self.grad_sync(self.model)
+        return loss.detach(), delta, self._last_q
+
+    def _step(self):
         if self.max_grad_norm is not None:
             clip_l2_grad_norm_(self.model.parameters(), self.max_grad_norm)
         self.optimizer.step()
-        return loss.detach(), delta
 
     def _learn_graphed(self, exp_batch, want_errors):
-        sig = tuple(sorted((k, tuple(v.shape), v.dtype) for k, v in exp_batch.items())) + (
-            want_errors,)
-        if self._graph is None:
-            if self._graph_warmup < 3:  # eager warm-up: optimizer state, cuDNN / cuBLAS plans
-                self._graph_warmup += 1
-                return self._learn(exp_batch, want_errors)
-            self._graph_sig = sig
-            self._static_in = {k: v.clone() for k, v in exp_batch.items()}
-            torch.cuda.synchronize(self.device)
-            self._graph = torch.cuda.CUDAGraph()
-            if self.grad_sync is None:
-                with torch.cuda.graph(self._graph):
-                    self._static_out = self._learn(self._static_in, want_errors)
-            else:
-                with torch.cuda.graph(self._graph):
-                    loss, delta = self._compute_loss(self._static_in, want_errors=want_errors)
-                    self.optimizer.zero_grad()
-                    loss.backward()
-                    self.grad_sync.pack(self.model)
-                    self._static_out = (loss.detach(), delta)
-                self._graph_step = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(self._graph_step, pool=self._graph.pool()):
-                    self.grad_sync.unpack(self.model)
-                    if self.max_grad_norm is not None:
-                        clip_l2_grad_norm_(self.model.parameters(), self.max_grad_norm)
-                    self.optimizer.step()
-            self._static_q = self._last_q
-        if sig != self._graph_sig:
-            return self._learn(exp_batch, want_errors)  # different batch layout: run eagerly
-        for k, v in exp_batch.items():
-            self._static_in[k].copy_(v)
-        self._graph.replay()  # capture only records: every update is a replay
-        if self.grad_sync is not None:
-            self.grad_sync.reduce(self.model)  # NCCL, eager, between the two graphs
-            self._graph_step.replay()
-        self._last_q = self._static_q
-        return self._static_out
+        self._graph.load((self.clip_delta, self.batch_accumulator, self.max_grad_norm,
+                          want_errors), exp_batch)
+        if self.grad_sync is None:
+            return self._graph.run(lambda b: self._learn(b, want_errors))
+
+        def backward_and_pack(b):
+            out = self._backward(b, want_errors)
+            self.grad_sync.pack(self.model)
+            return out
+
+        out = self._graph.run(backward_and_pack)
+        self.grad_sync.reduce(self.model)  # NCCL, eager, between the two graphs
+        self._step_graph.load(self._graph.key, {})
+
+        def unpack_and_step(_):
+            self.grad_sync.unpack(self.model)
+            self._step()
+
+        self._step_graph.run(unpack_and_step)
+        return out
 
     def _forward(self, model, exp_batch, key):
         """Q-values of exp_batch[key] ("state" / "next_state"); a recurrent model
@@ -409,33 +398,23 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
 
     def _greedy_graphed(self, batch_obs):
         """Acting forward (a few dozen tiny launches at num_envs images) replayed as one CUDA
-        graph: observations are copied into a static buffer, the greedy actions come back in
-        one.  Falls back to the eager call while warming up or when the batch layout changes."""
+        graph: observations are copied into a static buffer, the action values and greedy
+        actions come back in static ones.  None when the observations are not one tensor."""
         x = self.batch_states(batch_obs, self.device, self.phi)
         if not isinstance(x, torch.Tensor):
             return None
-        sig = (tuple(x.shape), x.dtype)
-        if self._act_graph is None:
-            if self._act_graph_warmup < 3:
-                self._act_graph_warmup += 1
-                return None
-            self._act_sig = sig
-            self._act_in = x.clone()
-            torch.cuda.synchronize(self.device)
-            self._act_graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self._act_graph):
-                self._act_av = self.model(self._act_in)
-                self._act_out = self._act_av.greedy_actions
-        if sig != self._act_sig:
-            return None
-        self._act_in.copy_(x)
-        self._act_graph.replay()
-        return self._act_av, self._act_out
+        self._act_graph.load((), {"x": x})
+
+        def greedy(b):
+            av = self.model(b["x"])
+            return av, av.greedy_actions
+
+        return self._act_graph.run(greedy)
 
     def batch_act(self, batch_obs):
         with torch.no_grad(), evaluating(self.model):
             graphed = None
-            if self._graph_enabled and type(self)._evaluate_model is DQN._evaluate_model:
+            if self._act_graph is not None and type(self)._evaluate_model is DQN._evaluate_model:
                 graphed = self._greedy_graphed(batch_obs)
             if graphed is not None:
                 batch_av, greedy = graphed
@@ -529,9 +508,9 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
         exp_batch = batch_recurrent_experiences(
             episodes, device=self.device, phi=self.phi, gamma=self.gamma,
             batch_states=self.batch_states)
-        loss, _ = self._learn(exp_batch, want_errors=False)
-        self.loss_record.append(loss.detach())
-        self.q_record.extend(self._last_q)
+        loss, _, q = self._learn(exp_batch, want_errors=False)
+        self.loss_record.append(loss)
+        self.q_record.extend(q)
         self.optim_t += 1
 
     def save_snapshot(self, dirname):

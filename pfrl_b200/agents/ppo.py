@@ -43,12 +43,13 @@ import torch.nn.functional as F
 from torch.nn.utils.rnn import PackedSequence
 
 from pfrl_b200 import agent
+from pfrl_b200.agents._graph import CapturedStep
 from pfrl_b200.agents.dqn import _DeviceRing
 from pfrl_b200.agents.soft_actor_critic import mode_of_distribution
 from pfrl_b200.ops import ppo as fused
 from pfrl_b200.ops import rollout
 from pfrl_b200.utils.batch_states import batch_states
-from pfrl_b200.utils.modes import evaluating, no_distribution_validation
+from pfrl_b200.utils.modes import evaluating
 from pfrl_b200.utils.recurrent import (
     concatenate_recurrent_states, flatten_sequences_time_first, mask_recurrent_state_at,
     one_step_forward, pack_and_forward,
@@ -403,14 +404,9 @@ class PPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
         # Optional: the minibatch step (gather, forward, fused loss, backward, clip,
         # Adam: ~100 launches of tiny kernels, 320 times per update) replayed as ONE
         # CUDA graph over persistent dataset buffers.
-        self._graph_enabled = bool(cuda_graph) and self.device.type == "cuda" \
-            and grad_sync is None
         self._graph = None
-        self._graph_key = None
-        if self._graph_enabled:
-            for group in optimizer.param_groups:
-                if "capturable" in group:
-                    group["capturable"] = True
+        if cuda_graph and self.device.type == "cuda" and grad_sync is None:
+            self._graph = CapturedStep(3, (optimizer,))
         # rollout (device tensors per vector step)
         self._rollout_clear()
         self._cur_state = None
@@ -519,16 +515,16 @@ class PPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
             norm.experience(flat_s)
 
         adv_stats = stats if self.standardize_advantages else None
-        if self._graph_enabled:
+        if self._graph is not None:
             self._minibatches_graphed(order, flat_s, flat_a, log_probs_old, v_old, adv, v_teacher,
                                       adv_stats)
         else:
             for mb in _yield_minibatch_indices(order, self.minibatch_size, self.epochs):
                 idx = torch.as_tensor(mb, device=dev)
                 s = flat_s[idx]
-                self._minibatch_step(norm(s, update=False) if norm else s, flat_a[idx],
-                                     log_probs_old[idx], v_old[idx], adv[idx], v_teacher[idx],
-                                     adv_stats)
+                self._record_losses(self._minibatch_step(
+                    norm(s, update=False) if norm else s, flat_a[idx], log_probs_old[idx],
+                    v_old[idx], adv[idx], v_teacher[idx], adv_stats))
                 self.n_updates += 1
 
         self._explained_variance_from(v_teacher, v_old)
@@ -631,10 +627,11 @@ class PPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
                 (distribs, vs_pred), _ = pack_and_forward(
                     self.model, PackedSequence(s, batch_sizes), rs.get(0))
                 self.model.zero_grad()
-                loss = self._lossfun(
+                loss, parts = self._lossfun(
                     distribs.entropy(), vs_pred, distribs.log_prob(a),
                     vs_pred_old=vo_mb[..., None], log_probs_old=lp_mb, advs=adv_mb,
                     vs_teacher=vt_mb[..., None], adv_stats=adv_stats)
+                self._record_losses(parts)
                 loss.backward()
                 if self.max_grad_norm is not None:
                     torch.nn.utils.clip_grad_norm_(self.model.parameters(), self.max_grad_norm)
@@ -645,77 +642,62 @@ class PPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
         self._rollout_clear(E)
         self._rstates, self._rpresent = [], []
 
-    def _minibatch_step(self, s, a, log_probs_old, v_old, advs, v_teacher, adv_stats,
-                        record=True):
-        """One gradient step on one minibatch (ppo.py:480-532)."""
+    def _minibatch_step(self, s, a, log_probs_old, v_old, advs, v_teacher, adv_stats):
+        """One gradient step on one minibatch (ppo.py:480-532); returns the detached
+        (policy loss, value loss)."""
         distribs, vs_pred = self.model(s)
         self.model.zero_grad()
-        loss = self._lossfun(
+        loss, parts = self._lossfun(
             distribs.entropy(), vs_pred, distribs.log_prob(a), vs_pred_old=v_old[..., None],
             log_probs_old=log_probs_old, advs=advs, vs_teacher=v_teacher[..., None],
-            adv_stats=adv_stats, record=record)
+            adv_stats=adv_stats)
         loss.backward()
         if self.grad_sync is not None:
             self.grad_sync(self.model)
         if self.max_grad_norm is not None:
             torch.nn.utils.clip_grad_norm_(self.model.parameters(), self.max_grad_norm)
         self.optimizer.step()
+        return parts
+
+    def _record_losses(self, parts):
+        self.policy_loss_record.append(parts[0])
+        self.value_loss_record.append(parts[1])
 
     def _minibatches_graphed(self, order, flat_s, flat_a, log_probs_old, v_old, adv, v_teacher,
                              adv_stats):
-        dev, norm = self.device, self.obs_normalizer
+        """The minibatch steps over persistent dataset buffers, loaded once per update; each
+        row writes its minibatch's indices into the index buffer and runs the step."""
+        norm = self.obs_normalizer
+        mbs = list(_yield_minibatch_indices(order, self.minibatch_size, self.epochs))
+        all_idx = torch.as_tensor(np.asarray(mbs, dtype=np.int64), device=self.device)
         # the normaliser is frozen during the epochs (update=False): apply it once
         data = dict(s=norm(flat_s, update=False) if norm else flat_s, a=flat_a,
-                    lp=log_probs_old, vo=v_old, adv=adv, vt=v_teacher)
+                    lp=log_probs_old, vo=v_old, adv=adv, vt=v_teacher, idx=all_idx[0])
         if adv_stats is not None:
             data["stats"] = adv_stats
-        mbs = list(_yield_minibatch_indices(order, self.minibatch_size, self.epochs))
-        all_idx = torch.as_tensor(np.asarray(mbs, dtype=np.int64), device=dev)
-        key = tuple((k, tuple(v.shape), v.dtype) for k, v in data.items()) + (self.minibatch_size,)
-        if self._graph_key != key:  # (re)allocate the persistent buffers, drop the old graph
-            self._graph, self._graph_key = None, key
-            self._g = {k: torch.empty_like(v) for k, v in data.items()}
-            self._g_idx = torch.zeros(self.minibatch_size, dtype=torch.int64, device=dev)
-            self._g_warm = 0
-        for k, v in data.items():
-            self._g[k].copy_(v)
-        g = self._g
+        g = self._graph.load((self.clip_eps, self.clip_eps_vf, self.value_func_coef,
+                              self.entropy_coef, self.max_grad_norm, self.minibatch_size), data)
 
-        def step(record):
-            i = self._g_idx
-            self._minibatch_step(g["s"][i], g["a"][i], g["lp"][i], g["vo"][i], g["adv"][i],
-                                 g["vt"][i], g.get("stats"), record=record)
+        def step(g):
+            i = g["idx"]
+            return self._minibatch_step(g["s"][i], g["a"][i], g["lp"][i], g["vo"][i],
+                                        g["adv"][i], g["vt"][i], g.get("stats"))
 
-        for row in range(all_idx.shape[0]):
-            self._g_idx.copy_(all_idx[row])
-            if self._graph is None and self._g_warm < 3:
-                self._g_warm += 1
-                step(record=True)
-            else:
-                if self._graph is None:
-                    torch.cuda.synchronize(dev)
-                    self._graph = torch.cuda.CUDAGraph()
-                    with no_distribution_validation(), torch.cuda.graph(self._graph):
-                        step(record=False)
-                # capture only records the work: every row (this one included) is replayed
-                self._graph.replay()
-                self.policy_loss_record.append(self._last_loss_parts[1])
-                self.value_loss_record.append(self._last_loss_parts[2])
+        for row in all_idx:
+            g["idx"].copy_(row)
+            self._record_losses(self._graph.run(step))
             self.n_updates += 1
 
     def _lossfun(self, entropy, vs_pred, log_probs, vs_pred_old, log_probs_old, advs, vs_teacher,
-                 adv_stats=None, record=True):
-        """ppo.py:495 + :634-671."""
+                 adv_stats=None):
+        """ppo.py:495 + :634-671; returns the loss and the detached (policy loss, value
+        loss)."""
         if self.use_fused and log_probs.is_cuda:
             loss, parts = fused.ppo_loss(
                 log_probs, entropy, vs_pred, log_probs_old, vs_pred_old, advs, vs_teacher,
                 adv_stats, self.clip_eps, self.clip_eps_vf, self.value_func_coef,
                 self.entropy_coef)
-            self._last_loss_parts = parts  # static tensor when graph-captured
-            if record:
-                self.policy_loss_record.append(parts[1])
-                self.value_loss_record.append(parts[2])
-            return loss
+            return loss, (parts[1], parts[2])
         if adv_stats is not None:
             advs = (advs - adv_stats[0]) / (adv_stats[1] + 1e-8)
         prob_ratio = torch.exp(log_probs - log_probs_old)
@@ -731,13 +713,9 @@ class PPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
                 F.mse_loss(vs_pred, vs_teacher, reduction="none"),
                 F.mse_loss(clipped, vs_teacher, reduction="none")))
         loss_entropy = -torch.mean(entropy)
-        self._last_loss_parts = torch.stack(
-            [loss_policy.detach() * 0, loss_policy.detach(), loss_value_func.detach()])
-        if record:
-            self.value_loss_record.append(loss_value_func.detach())
-            self.policy_loss_record.append(loss_policy.detach())
-        return (loss_policy + self.value_func_coef * loss_value_func
+        loss = (loss_policy + self.value_func_coef * loss_value_func
                 + self.entropy_coef * loss_entropy)
+        return loss, (loss_policy.detach(), loss_value_func.detach())
 
     def get_statistics(self):
         if self.explained_variance is None:

@@ -16,11 +16,12 @@ from torch import nn
 from torch.nn import functional as F
 
 from pfrl_b200.agent import AttributeSavingMixin, BatchAgent
+from pfrl_b200.agents._graph import CapturedStep
 from pfrl_b200.agents.dqn import _DeviceRing
 from pfrl_b200.replay_buffer import ReplayUpdater, batch_experiences
 from pfrl_b200.utils import clip_l2_grad_norm_
 from pfrl_b200.utils.batch_states import batch_states
-from pfrl_b200.utils.modes import evaluating, no_distribution_validation
+from pfrl_b200.utils.modes import evaluating
 from pfrl_b200.utils.copy_param import synchronize_parameters
 from pfrl_b200.utils.mode_of_distribution import mode_of_distribution  # NOQA (re-exported)
 
@@ -107,18 +108,10 @@ class SoftActorCritic(AttributeSavingMixin, BatchAgent):
         self.n_policy_updates = 0
         # Optional: replay the whole update (5 small networks, 4 optimizers, 2
         # Polyak steps: ~300 launches of tiny kernels) as ONE CUDA graph.
-        self._graph_enabled = bool(cuda_graph) and self.device.type == "cuda" \
-            and grad_sync is None
         self._graph = None
-        self._graph_warmup = 0
-        if self._graph_enabled:
-            for opt in (policy_optimizer, q_func1_optimizer, q_func2_optimizer,
-                        self.temperature_optimizer):
-                if opt is None:
-                    continue
-                for group in opt.param_groups:
-                    if "capturable" in group:
-                        group["capturable"] = True
+        if cuda_graph and self.device.type == "cuda" and grad_sync is None:
+            self._graph = CapturedStep(3, (policy_optimizer, q_func1_optimizer,
+                                           q_func2_optimizer, self.temperature_optimizer))
 
     @property
     def temperature(self):
@@ -220,28 +213,13 @@ class SoftActorCritic(AttributeSavingMixin, BatchAgent):
 
     _GRAPH_KEYS = ("state", "next_state", "action", "reward", "discount", "is_state_terminal")
 
-    def _update_graphed(self, batch):
-        if self._graph is None:
-            if self._graph_warmup < 3:  # eager warm-up (optimizer state, cuBLAS workspaces)
-                self._graph_warmup += 1
-                return self._update_core(batch)
-            self._static_in = {k: batch[k].clone() for k in self._GRAPH_KEYS}
-            self._graph_shapes = {k: v.shape for k, v in self._static_in.items()}
-            torch.cuda.synchronize(self.device)
-            self._graph = torch.cuda.CUDAGraph()
-            with no_distribution_validation(), torch.cuda.graph(self._graph):
-                self._static_out = self._update_core(self._static_in)
-        if any(batch[k].shape != self._graph_shapes[k] for k in self._GRAPH_KEYS):
-            return self._update_core(batch)  # odd-sized batch: run eagerly
-        for k in self._GRAPH_KEYS:
-            self._static_in[k].copy_(batch[k])
-        self._graph.replay()  # capture only records: every update is a replay
-        return self._static_out
-
     def update(self, experiences, errors_out=None):
         batch = batch_experiences(experiences, self.device, self.phi, self.gamma)
-        if self._graph_enabled:
-            q1, q2, l1, l2, entropy = self._update_graphed(batch)
+        if self._graph is not None:
+            self._graph.load((self.soft_update_tau, self.max_grad_norm, self.entropy_target,
+                              self.initial_temperature if self.entropy_target is None else None),
+                             {k: batch[k] for k in self._GRAPH_KEYS})
+            q1, q2, l1, l2, entropy = self._graph.run(self._update_core)
         else:
             q1, q2, l1, l2, entropy = self._update_core(batch)
         self.n_policy_updates += 1

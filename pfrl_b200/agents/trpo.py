@@ -37,6 +37,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from pfrl_b200 import agent
+from pfrl_b200.agents._graph import CapturedStep
 from pfrl_b200.agents.dqn import _DeviceRing
 from pfrl_b200.agents.ppo import (  # NOQA
     _DeviceRollout, _compute_explained_variance, _make_dataset, _yield_minibatch_indices,
@@ -217,14 +218,11 @@ class TRPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
         self._policy_kind = None  # the kernels' distribution kind, False if not covered
         # Optional (cuda_graph=True): the value-function minibatch step and the fused policy
         # update (fixed shapes for a given N, CG iterations and backtracks) are each
-        # captured once and replayed
-        self._graph_enabled = bool(cuda_graph) and self.device.type == "cuda"
-        self._vf_graph = self._vf_graph_key = None
-        self._policy_graph = self._policy_graph_key = None
-        if self._graph_enabled:
-            for group in vf_optimizer.param_groups:
-                if "capturable" in group:
-                    group["capturable"] = True
+        # captured and replayed
+        self._vf_graph = self._policy_graph = None
+        if cuda_graph and self.device.type == "cuda":
+            self._vf_graph = CapturedStep(3, (vf_optimizer,))
+            self._policy_graph = CapturedStep(2)
 
     # ----------------------------------------------------------------- acting
     def batch_act(self, batch_obs):
@@ -290,7 +288,7 @@ class TRPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
         mbs = list(_yield_minibatch_indices(order, self.vf_batch_size, self.vf_epochs))
         # every minibatch has vf_batch_size indices: one upload for the whole stream
         all_idx = torch.as_tensor(np.asarray(mbs, dtype=np.int64), device=self.device)
-        if self._graph_enabled:
+        if self._vf_graph is not None:
             self._update_vf_graphed(obs, v_teacher, all_idx)
             return
         for i in all_idx:
@@ -306,35 +304,13 @@ class TRPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
         self.vf_optimizer.step()
 
     def _update_vf_graphed(self, obs, v_teacher, all_idx):
-        """The minibatch steps over persistent buffers: three eager, then one captured step
-        replayed for every remaining minibatch (PPO._minibatches_graphed)."""
-        key = (tuple(obs.shape), obs.dtype, self.vf_batch_size)
-        if self._vf_graph_key != key:  # (re)allocate the persistent buffers, drop the graph
-            self._vf_graph, self._vf_graph_key = None, key
-            self._vg = dict(obs=torch.empty_like(obs), vt=torch.empty_like(v_teacher),
-                            idx=torch.zeros(self.vf_batch_size, dtype=torch.int64,
-                                            device=self.device))
-            self._vf_warm = 0
-        g = self._vg
-        g["obs"].copy_(obs)
-        g["vt"].copy_(v_teacher)
-
-        def step():
-            self._vf_step(g["obs"][g["idx"]], g["vt"][g["idx"]])
-
+        """The minibatch steps over persistent buffers, loaded once per update
+        (PPO._minibatches_graphed)."""
+        g = self._vf_graph.load((self.max_grad_norm, self.vf_batch_size),
+                                dict(obs=obs, vt=v_teacher, idx=all_idx[0]))
         for row in all_idx:
             g["idx"].copy_(row)
-            if self._vf_graph is None and self._vf_warm < 3:
-                self._vf_warm += 1
-                step()
-                continue
-            if self._vf_graph is None:
-                torch.cuda.synchronize(self.device)
-                self._vf_graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(self._vf_graph):
-                    step()
-            # capture only records the work: every row (this one included) is replayed
-            self._vf_graph.replay()
+            self._vf_graph.run(lambda g: self._vf_step(g["obs"][g["idx"]], g["vt"][g["idx"]]))
 
     def _compute_gain(self, log_prob, log_prob_old, entropy, advs):
         """Compute a gain to maximize."""
@@ -442,7 +418,7 @@ class TRPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
         kind = self._fused_kind(states)
         if kind is False:
             return False
-        if self._graph_enabled:
+        if self._policy_graph is not None:
             out = self._policy_kernels_graphed(kind, states, actions, log_prob_old, advs,
                                                adv_stats)
         else:
@@ -494,36 +470,16 @@ class TRPO(_DeviceRollout, agent.AttributeSavingMixin, agent.BatchAgent):
         return cand_out, gain_out, record
 
     def _policy_kernels_graphed(self, kind, states, actions, log_prob_old, advs, adv_stats):
-        """_policy_kernels over persistent input buffers: two eager updates, then one
-        captured update replayed.  The graph is captured again when a shape or a
-        hyperparameter baked into it changes."""
+        """_policy_kernels over persistent input buffers."""
         inputs = dict(s=states, a=actions, lp=log_prob_old, adv=advs)
         if adv_stats is not None:
             inputs["stats"] = adv_stats
-        key = tuple((k, tuple(v.shape), v.dtype) for k, v in inputs.items()) + (
-            kind, self.max_kl, self.entropy_coef, self.conjugate_gradient_max_iter,
-            self.conjugate_gradient_damping, self.line_search_max_backtrack)
-        if self._policy_graph_key != key:
-            self._policy_graph, self._policy_graph_key = None, key
-            self._pg = {k: torch.empty_like(v) for k, v in inputs.items()}
-            self._pg_warm = 0
-        g = self._pg
-        for k, v in inputs.items():
-            g[k].copy_(v)
-
-        def run():
-            return self._policy_kernels(kind, g["s"], g["a"], g["lp"], g["adv"], g.get("stats"))
-
-        if self._policy_graph is None and self._pg_warm < 2:
-            self._pg_warm += 1
-            return run()
-        if self._policy_graph is None:
-            torch.cuda.synchronize(self.device)
-            self._policy_graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self._policy_graph):
-                self._pg_out = run()
-        self._policy_graph.replay()
-        return self._pg_out
+        self._policy_graph.load((kind, self.max_kl, self.entropy_coef,
+                                 self.conjugate_gradient_max_iter,
+                                 self.conjugate_gradient_damping,
+                                 self.line_search_max_backtrack), inputs)
+        return self._policy_graph.run(lambda g: self._policy_kernels(
+            kind, g["s"], g["a"], g["lp"], g["adv"], g.get("stats")))
 
     def _fisher_vector_product(self, states, kind, dparams, old):
         """v -> J^T (M J v) + damping v at the current parameters: J v by forward-mode AD

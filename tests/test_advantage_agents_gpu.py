@@ -85,7 +85,7 @@ def _train(kind, fused_step=True, graph=False, steps=80):
         agent.batch_observe(obs, r, d, np.zeros(4, dtype=bool))
         obs = env.reset(np.logical_not(d))
     assert agent.optim_t > 200
-    assert (agent._graph is not None) == graph
+    assert (agent._graph is not None and agent._graph.graph is not None) == graph
     params = [p.detach().clone() for p in agent.model.parameters()]
     return indices, params, dict(agent.get_statistics()), rbuf
 

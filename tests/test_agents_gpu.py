@@ -173,7 +173,7 @@ def test_sac_on_device_env(use_graph):
     assert np.isfinite(stats["average_q_func1_loss"]) and np.isfinite(stats["average_entropy"])
     assert len(agent.replay_buffer) == 8 * 60
     if use_graph:
-        assert agent._graph is not None  # the update really ran as a captured graph
+        assert agent._graph.graph is not None  # the update really ran as a captured graph
 
 
 
@@ -256,7 +256,7 @@ def test_dqn_update_as_cuda_graph_matches_eager():
             agent.batch_observe(obs, r, d, np.zeros(4, dtype=bool))
             obs = env.reset(np.logical_not(d))
         assert agent.optim_t > 200
-        assert (agent._graph is not None) == graph
+        assert (agent._graph is not None and agent._graph.graph is not None) == graph
         res[graph] = ([p.detach().clone() for p in agent.model.parameters()],
                       dict(agent.get_statistics()))
     for a, b in zip(res[False][0], res[True][0]):

@@ -49,4 +49,4 @@ for env_dev in (dev, "cpu", dev):
         torch.cuda.synchronize(); t4 = time.perf_counter()
         t["act"] += t1 - t0; t["step"] += t2 - t1; t["observe"] += t3 - t2; t["reset"] += t4 - t3
     print("env on", env_dev, {k: round(v / n * 1e3, 3) for k, v in t.items()}, "ms per vector step;",
-          "act graph:", agent._act_graph is not None, "sig", getattr(agent, "_act_sig", None))
+          "act graph:", agent._act_graph.graph is not None, "key", agent._act_graph.key)
