@@ -1125,10 +1125,12 @@ __device__ __forceinline__ void tree_update_multi(const UpdateArgs &a, unsigned 
 //     the exact tree has caught up and run the reference's arithmetic on it (the
 //     v5 code).  Never wrong, only slow; the count is reported
 //     (b2rl_per_info.scout_hits: fast | slow << 16).
-//   * the ascent warp applies draw k to the EXACT tree (shared-memory top +
-//     global bottom) with the reference's bottom-up adds, one draw after the
-//     other, a few draws behind.  The tree that goes back to HBM and every
-//     priority returned are exact.
+//   * the ascent warps apply draw k to the EXACT tree (shared-memory top +
+//     global bottom) with the reference's bottom-up adds, a few draws behind;
+//     draw k on warp k % V6_NASC, so draws of different level-12 subtrees are
+//     applied concurrently (draws of the same subtree never are: see the conflict
+//     test above).  The tree that goes back to HBM and every priority returned
+//     are exact.
 //   * seven scout warps; a publisher warp moves results out.
 // tools/v6_model.py is a CPU model of the decision logic (adversarial trees:
 // ties, 1e-30..1e+30 dynamic range, u on boundaries, mispredictions).
@@ -1136,20 +1138,27 @@ __device__ __forceinline__ void tree_update_multi(const UpdateArgs &a, unsigned 
 static constexpr int V6_NSCOUT = 7;
 static constexpr int V6_LAG = 6;
 static constexpr int V6_NBUF = 8;
-static constexpr int V6_Q = 16;
 static constexpr int V6_NTOP = 1 << (V6_T - 1);  // 4096 level-12 nodes
 // Warp roles.  The issue arbiter of an SM sub-partition (warp id % 4) prefers its
-// highest eligible warp id, so the latency-critical main warp gets a sub-partition to
-// itself, the ascent warp shares its own with idle warps only, and the scouts fill
-// sub-partition 0 (warps 0, 4, 8, 12), then sub-partition 2 beside the publisher (warps 6,
-// 10, 14).  Seven scouts, each working on every seventh draw, can start a draw V6_LAG = 6
-// draws ahead; four could not start before they finished the draw four back.
-static constexpr int V6_W_MAIN = 3, V6_W_ASC = 1, V6_W_PUB = 2;
+// highest eligible warp id, so the latency-critical main warp gets sub-partition 3 to
+// itself (warps 7, 11, 15 stay idle), the V6_NASC ascent warps take sub-partition 1 (warps
+// 1, 5, ...; the others stay idle), and the scouts fill sub-partition 0 (warps 0, 4, 8,
+// 12), then sub-partition 2 beside the publisher (warps 6, 10, 14).  Seven scouts, each
+// working on every seventh draw,
+// can start a draw V6_LAG = 6 draws ahead; four could not start before they finished the
+// draw four back.  Ascent warp i applies draws k = i (mod V6_NASC) in order: one warp had
+// 715 cycles of work per draw against the main warp's 517 and could fall behind it.
+static constexpr int V6_NASC = 2;
+static constexpr int V6_W_MAIN = 3, V6_W_PUB = 2;
 __device__ __forceinline__ int v6_scout_id(int warp)
 {
     if ((warp & 3) == 0) return warp >> 2;
     if ((warp & 3) == 2 && warp != V6_W_PUB) return 3 + (warp >> 2);
     return -1;
+}
+__device__ __forceinline__ int v6_ascent_id(int warp)
+{
+    return ((warp & 3) == 1 && (warp >> 2) < V6_NASC) ? warp >> 2 : -1;
 }
 static constexpr int V6_THREADS = 512;
 
@@ -1201,23 +1210,31 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
     constexpr int NIT = (PAIRS + 31) / 32;
     constexpr int CHUNK = 32;
     constexpr int NSCOUT = V6_NSCOUT, LAG = V6_LAG, NBUF = V6_NBUF, RING = EX_RING;
-    constexpr int Q = V6_Q;
-    // F_ASC:  draws whose exact update is VISIBLE (global stores fenced), published in
-    //         batches -- the fence waits for the L2 acknowledgement of the ascent's global
-    //         stores and a MEMBAR holds up the SM's shared-memory pipe for everybody, so it
-    //         must not be paid per draw;
-    // F_ASCR: draws the ascent warp has finished READING the inputs of (relaxed, per draw):
-    //         staged buffers and queue slots can be reused.
-    constexpr int F_MAIN = 24, F_ASC = 25, F_PUB = 26, F_ASCR = 27;
-    constexpr int ASC_BATCH = 4;
+    constexpr int NASC = V6_NASC;
+    // Progress of the ascent warps, one word per warp i, each the next draw of that warp
+    // (n once it has none left); the draws before the MINIMUM over the warps are done:
+    // F_ASC + i:  draws whose exact update is VISIBLE (global stores fenced), published in
+    //             batches -- the fence waits for the L2 acknowledgement of the ascent's global
+    //             stores and a MEMBAR holds up the SM's shared-memory pipe for everybody, so it
+    //             must not be paid per draw;
+    // F_ASCR + i: draws whose inputs the warp has finished READING (relaxed, per draw): a
+    //             scout waits for the warp that read the buffer it is about to restage.
+    // A reader of F_ASC acquires every warp's word: the minimum of relaxed loads would not
+    // order it after the stores of the warp that applied a given draw.
+    constexpr int F_MAIN = 24, F_PUB = 26, F_ASC = 0, F_ASCR = 8;
+    // fence every ASC_BATCH draws of a warp: the fenced prefix lags by up to NASC * ASC_BATCH
+    // draws, and a scout that stages a subtree still in flight costs a slow draw
+    constexpr int ASC_BATCH = 2;
     static_assert(D >= 5 && D <= 9, "v6 stages 5..9 levels per draw");
     static_assert(NSCOUT >= 1 && NSCOUT <= 7, "scout warps: 0, 4, 8, 12, 6, 10, 14");
+    static_assert(NASC >= 1 && NASC <= 4, "ascent warps: 1, 5, 9, 13");
     static_assert(NBUF <= 8, "ready64 has 8 words");
+    static_assert(NBUF < RING, "the ascent lags the main warp by at most NBUF draws");
     double *etop = smem_d;                      // exact top, levels 0..12
     double *mtab = etop + TOPN;                 // [NTOP] approximate node mass, descent order
     double *plo = mtab + NTOP;                  // [NTOP] approximate prefix inside a block of 64
     double *phi = plo + NTOP;                   // [64]   approximate prefix of the blocks
-    double *s_misc = phi + 64;                  // [8]: rootA, total, min-root
+    double *s_misc = phi + 64;                  // [8]: rootA, total, min-root, ascent cycles (2)
     // [NBUF] one word per staged buffer: draw << 32 | F_ASC seen << 12 | node (descent order)
     unsigned long long *ready64 = reinterpret_cast<unsigned long long *>(s_misc + 8);
     double *sub_own = s_misc + 16;
@@ -1236,13 +1253,20 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
     unsigned short *lastd = reinterpret_cast<unsigned short *>(bar + 2 + NBUF);
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
+    // draws [0, result) whose exact update every ascent warp has fenced
+    auto asc_fenced = [&]() {
+        int m = ld_acquire_smem(&flags[F_ASC]);
+#pragma unroll
+        for (int i = 1; i < NASC; i++) m = min(m, ld_acquire_smem(&flags[F_ASC + i]));
+        return m;
+    };
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < 32; i++) flags[i] = -1;
         flags[F_MAIN] = 0;
-        flags[F_ASC] = 0;
-        flags[F_ASCR] = 0;
+        for (int i = 0; i < NASC; i++) flags[F_ASC + i] = flags[F_ASCR + i] = i < a.n ? i : a.n;
         flags[F_PUB] = 0;
+        s_misc[3] = s_misc[4] = 0.0; // as integers: the ascent warps' clock64 sums
         mbar_init(bar, 1);
         for (int i = 0; i < NBUF; i++) mbar_init(bar + 2 + i, 1);
         mbar_fence_init();
@@ -1304,9 +1328,10 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             const double uk = u_next;
             if (k + NSCOUT < a.n) u_next = a.u[k + NSCOUT];
             const int b = k % NBUF;
+            const int kb = k - NBUF; // the draw buffer b was staged for last: its ascent read it
             int m;
             while ((m = ld_acquire_smem(&flags[F_MAIN])) < k - LAG ||
-                   ld_acquire_smem(&flags[F_ASCR]) < k - NBUF + 1)
+                   (kb >= 0 && ld_acquire_smem(&flags[F_ASCR + kb % NASC]) <= kb))
                 __nanosleep(32);
             const long long tc1 = V6_CLK();
             // ---- prediction (any error only costs a slow draw): search the tables
@@ -1321,7 +1346,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             const int ord = 64 * blk + w;
             pos -= plo[ord];
             const unsigned unode = (unsigned)(NTOP + (ord ^ oflip));
-            const int seen = ld_acquire_smem(&flags[F_ASC]);
+            const int seen = asc_fenced();
             double *dst = sub_pref + b * BUFN;
             // ---- one bulk copy per level: the 2^j nodes j levels below `unode` are contiguous
             uint64_t *sb = bar + 2 + b;
@@ -1500,7 +1525,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                 if (!fast) {
                     // ---- slow path: the reference's arithmetic on the exact tree
                     nslow++;
-                    while (ld_acquire_smem(&flags[F_ASC]) < k) {
+                    while (asc_fenced() < k) {
                     }
                     // the ascent warp keeps level 12 exact; levels 11..0 = fl(left + right)
                     for (int lv = T - 2; lv >= 0; lv--) {
@@ -1538,10 +1563,12 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                 }
                 const long long tm2 = V6_CLK();
                 rootA = rootA - prio;
-                // room in the ascent queue: Q entries, checked every fourth draw
-                if ((k & 3) == 0)
-                    while (ld_acquire_smem(&flags[F_ASCR]) < k - Q + 4) {
-                    }
+                // No wait for room in the ascent queue: every draw j < k - NBUF has been read
+                // by its ascent warp already.  Draw j + NBUF was decided either fast, on the
+                // staging of a scout that waited for that read before reusing buffer j % NBUF,
+                // or slow, after every earlier draw was fenced.  So the ring slot written
+                // below (RING > NBUF draws back) is free.  The check cost this warp ~60 cycles
+                // per draw: its acquire load queued behind the previous draw's stores.
                 const long long tm3 = V6_CLK();
                 // ---- loads first: this draw's table entries
                 const int base = ord & ~63, within = ord & 63, bk = ord >> 6;
@@ -1591,10 +1618,14 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             a.dbg_cycles[4] = c_stores;
         }
         if (lane == 0) a.st->pad = (nfast & 0xffff) | (nslow << 16); // fast draws, slow draws
-    } else if (warp == V6_W_ASC) {
+    } else if (v6_ascent_id(warp) >= 0) {
         // --------------- ascent: _write(ix, 0.0) on the exact tree ---------------
+        // Draws in flight on different warps touch disjoint nodes: a fast draw at node o is
+        // accepted only if every earlier draw at o is inside the fenced prefix its scout read
+        // before copying, and a slow draw waits for all earlier draws to be fenced.
+        const int ai = v6_ascent_id(warp);
         long long c_await = 0, c_awork = 0;
-        for (int k = 0; k < a.n; k++) {
+        for (int k = ai; k < a.n; k += NASC) {
             const long long ta0 = V6_CLK();
             while (ld_acquire_smem(&flags[F_MAIN]) <= k) __nanosleep(20);
             const long long ta1 = V6_CLK();
@@ -1628,15 +1659,17 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             }
             __syncwarp();
             if (lane == 0) {
+                const int next = k + NASC < a.n ? k + NASC : a.n; // this warp's next draw
                 // inputs consumed: a plain store ordered after the loads that fed the chain
-                *reinterpret_cast<volatile int *>(&flags[F_ASCR]) = k + 1;
-                // visibility of the global stores: every ASC_BATCH draws, and whenever
-                // the main warp has nothing more queued (it may be waiting for us)
-                if ((k + 1) % ASC_BATCH == 0 || k + 1 == a.n ||
-                    *reinterpret_cast<volatile int *>(&flags[F_MAIN]) == k + 1) {
+                *reinterpret_cast<volatile int *>(&flags[F_ASCR + ai]) = next;
+                // visibility of the global stores: every ASC_BATCH draws of this warp, and
+                // whenever the main warp has decided nothing beyond this warp's next draw (it
+                // may be waiting for us in the slow path while we wait for that draw)
+                if ((k / NASC + 1) % ASC_BATCH == 0 || next == a.n ||
+                    *reinterpret_cast<volatile int *>(&flags[F_MAIN]) <= next) {
                     // the scouts read the bottom levels with the bulk-copy engine (async proxy)
                     asm volatile("fence.proxy.async;" ::: "memory");
-                    st_release_smem(&flags[F_ASC], k + 1);
+                    st_release_smem(&flags[F_ASC + ai], next);
                 }
             }
             __syncwarp();
@@ -1644,8 +1677,8 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             c_awork += V6_CLK() - ta1;
         }
         if (a.dbg_cycles && lane == 0) {
-            a.dbg_cycles[16] = c_await;
-            a.dbg_cycles[17] = c_awork;
+            atomicAdd(reinterpret_cast<unsigned long long *>(&s_misc[3]), (unsigned long long)c_await);
+            atomicAdd(reinterpret_cast<unsigned long long *>(&s_misc[4]), (unsigned long long)c_awork);
         }
     } else if (warp == V6_W_PUB) {
         // ----------------------------- publisher -----------------------------
@@ -1675,6 +1708,10 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
         }
     }
     __syncthreads();
+    if (a.dbg_cycles && threadIdx.x == 0) { // summed over the ascent warps: cycles per draw / B
+        a.dbg_cycles[16] = *reinterpret_cast<const long long *>(&s_misc[3]);
+        a.dbg_cycles[17] = *reinterpret_cast<const long long *>(&s_misc[4]);
+    }
     // levels 11..0 of the exact top from level 12 (see the ascent warp)
     for (int lv = T - 2; lv >= 0; lv--) {
         const int wdt = 1 << lv;
