@@ -364,7 +364,7 @@ int b2rl_replay_step(b2rl_replay *h, const b2rl_step_args *args, void *stream);
  * [31..35] phases of the multi-CTA write-back in ns since CTA 0's entry: entries collected,
  * subtree stored, arrival ticket taken (all CTA 0), subtree roots loaded, completion flag
  * released (last CTA); with B2RL_WB_FINE=1 in the environment also [28..30]: CTA 0's sort /
- * unique done, siblings fetched, level loop done.  out_ns_host has 36 entries.  Measurement aid (bench.py, tools/v6_cycles.py). */
+ * unique done, siblings fetched, level loop done.  out_ns_host has 36 entries.  Measurement aid (bench.py, tools/v6_pipeline.py). */
 int b2rl_step_times(b2rl_replay *h, uint64_t *out_ns_host, void *stream);
 
 /* Answer the last sample with TD errors on the device WITHOUT launching: the

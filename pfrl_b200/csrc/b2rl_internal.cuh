@@ -30,6 +30,13 @@ void b2rl_set_error(const char *fmt, ...);
         }                                                                      \
     } while (0)
 
+// pass a failing B2RL status of an internal call on to the caller
+#define TRY(x)                                                                 \
+    do {                                                                       \
+        int rc__ = (x);                                                        \
+        if (rc__ != B2RL_OK) return rc__;                                      \
+    } while (0)
+
 // ---- device-side scalar state ----------------------------------------------
 // Lives in HBM so that kernels never need host-supplied counters; the host
 // keeps mirrors for the (deterministic) host-driven paths.

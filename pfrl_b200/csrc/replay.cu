@@ -223,12 +223,6 @@ static int dev_alloc(b2rl_replay *h, T **p, size_t count)
     return B2RL_OK;
 }
 
-#define TRY(x)                                                                 \
-    do {                                                                       \
-        int rc__ = (x);                                                        \
-        if (rc__ != B2RL_OK) return rc__;                                      \
-    } while (0)
-
 static int create_impl(b2rl_replay *h)
 {
     const b2rl_replay_config &c = h->cfg;

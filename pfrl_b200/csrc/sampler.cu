@@ -23,12 +23,6 @@
 
 #include "tree_dev.cuh"
 
-#define TRY(x)                                                                 \
-    do {                                                                       \
-        int rc__ = (x);                                                        \
-        if (rc__ != B2RL_OK) return rc__;                                      \
-    } while (0)
-
 extern __shared__ __align__(128) unsigned char smem_raw[];
 
 __global__ void __launch_bounds__(256, 1) k_sample_exact(SampleArgs a)
@@ -59,33 +53,25 @@ static cudaError_t launch_sample(const SampleArgs &a, int mode, cudaStream_t s)
 {
     const SamplerChoice c = choose_sampler(mode, a.levels, a.n);
     const size_t smem = sampler_smem_bytes(c, a);
-    switch (c.kind) {
-    case SAMPLER_V6:
-        return with_depth<5, 9>(c.D, [&](auto d) {
-            constexpr int D = decltype(d)::value;
+    return with_sampler(c, [&](auto d, auto kind) {
+        constexpr int D = decltype(d)::value, KIND = decltype(kind)::value;
+        if constexpr (KIND == SAMPLER_V6) {
             const cudaError_t e = b2rl_allow_smem<k_sample_exact_v6<D>>(smem);
             if (e != cudaSuccess) return e;
             k_sample_exact_v6<D><<<1, V6_THREADS, smem, s>>>(a);
-            return cudaGetLastError();
-        });
-    case SAMPLER_V5:
-        return with_depth<1, 10>(c.D, [&](auto d) {
-            constexpr int D = decltype(d)::value;
+        } else if constexpr (KIND == SAMPLER_V5) {
             const cudaError_t e = b2rl_allow_smem<k_sample_exact_deep<D>>(smem);
             if (e != cudaSuccess) return e;
             k_sample_exact_deep<D><<<1, 128, smem, s>>>(a);
-            return cudaGetLastError();
-        });
-    case SAMPLER_SMALL: {
-        const cudaError_t e = b2rl_allow_smem<k_sample_exact>(200 * 1024);
-        if (e != cudaSuccess) return e;
-        k_sample_exact<<<1, 256, smem, s>>>(a);
+        } else if constexpr (KIND == SAMPLER_SMALL) {
+            const cudaError_t e = b2rl_allow_smem<k_sample_exact>(200 * 1024);
+            if (e != cudaSuccess) return e;
+            k_sample_exact<<<1, 256, smem, s>>>(a);
+        } else {
+            k_sample_parallel<<<1, 512, smem, s>>>(a);
+        }
         return cudaGetLastError();
-    }
-    default:
-        k_sample_parallel<<<1, 512, smem, s>>>(a);
-        return cudaGetLastError();
-    }
+    });
 }
 
 static int v6_slow_every()

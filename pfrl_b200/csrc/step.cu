@@ -28,12 +28,6 @@
 
 #include "tree_dev.cuh"
 
-#define TRY(x)                                                                 \
-    do {                                                                       \
-        int rc__ = (x);                                                        \
-        if (rc__ != B2RL_OK) return rc__;                                      \
-    } while (0)
-
 static constexpr int GS = 8;            // stages of the part ring in shared memory
 static constexpr int PIECE_MAX = 8192;  // parts larger than this are cut in pieces
 static constexpr int STEP_THREADS = 512;
@@ -242,33 +236,19 @@ __global__ void __launch_bounds__(STEP_THREADS, 1) k_replay_step(const __grid_co
     if (threadIdx.x == 0) a.times[8 + blockIdx.x] = global_ns();
 }
 
-template <int D, int MODE>
-static cudaError_t launch_step_as(const StepArgs &a, int grid, size_t smem, cudaStream_t s)
-{
-    const cudaError_t e = b2rl_allow_smem<k_replay_step<D, MODE>>(227 * 1024);
-    if (e != cudaSuccess) return e;
-    k_replay_step<D, MODE><<<grid, STEP_THREADS, smem, s>>>(a);
-    return cudaGetLastError();
-}
-
 static cudaError_t launch_step(const StepArgs &a, int mode, int grid, size_t smem_other,
                                cudaStream_t s)
 {
     const SamplerChoice c = choose_sampler(mode, a.s.levels, a.s.n);
     const size_t sm = sampler_smem_bytes(c, a.s);
     const size_t smem = sm > smem_other ? sm : smem_other;
-    switch (c.kind) {
-    case SAMPLER_PARALLEL: return launch_step_as<0, SAMPLER_PARALLEL>(a, grid, smem, s);
-    case SAMPLER_SMALL: return launch_step_as<0, SAMPLER_SMALL>(a, grid, smem, s);
-    case SAMPLER_V6:
-        return with_depth<5, 9>(c.D, [&](auto d) {
-            return launch_step_as<decltype(d)::value, SAMPLER_V6>(a, grid, smem, s);
-        });
-    default:
-        return with_depth<1, 10>(c.D, [&](auto d) {
-            return launch_step_as<decltype(d)::value, SAMPLER_V5>(a, grid, smem, s);
-        });
-    }
+    return with_sampler(c, [&](auto d, auto kind) {
+        constexpr int D = decltype(d)::value, MODE = decltype(kind)::value;
+        const cudaError_t e = b2rl_allow_smem<k_replay_step<D, MODE>>(227 * 1024);
+        if (e != cudaSuccess) return e;
+        k_replay_step<D, MODE><<<grid, STEP_THREADS, smem, s>>>(a);
+        return cudaGetLastError();
+    });
 }
 
 // ---------------------------------------------------------------------------

@@ -1,8 +1,11 @@
 // tree_dev.cuh -- device-side building blocks on the dense fp64 heaps, shared
 // by the stand-alone kernels (sampler.cu) and the fused replay step (step.cu):
 //
+//   choose_sampler()       the sampler of a draw; with_sampler() its kernel
+//   descend_top<T>() ...   one copy each of the samplers' shared pieces
 //   exact_deep<D>()        bit-exact sequential sampler (main warp + two scout
 //                          warps + a publisher warp)
+//   exact_small()          bit-exact sampler, whole tree in shared memory
 //   exact_deep_v6<D>()     bit-exact sampler deciding on approximate tables
 //   sample_parallel()      all descents concurrently on the frozen tree
 //   tree_update_multi()    priority write-back for <= 512 leaves: sorted
@@ -51,7 +54,7 @@ struct SampleArgs {
     // path on every k-th draw / widen the decision margin; results must not change
     int dbg_slow_every;
     double dbg_eps_scale;
-    long long *dbg_cycles; // optional [32]: clock64 sums per pipeline segment (tools/v6_cycles.py)
+    long long *dbg_cycles; // optional [32]: clock64 sums per pipeline segment (tools/v6_pipeline.py)
 };
 
 // The sampler that serves a draw of n from a tree with leaves at heap level `levels`; the
@@ -75,15 +78,31 @@ inline SamplerChoice choose_sampler(int mode, int levels, int n)
     return {SAMPLER_V5, levels - (TOP_LEVELS - 1)};
 }
 
-// f(std::integral_constant<int, d>{}) for a runtime d in [LO, HI]: turns the depth of a
-// SamplerChoice into the template argument of the kernel that serves it.
-template <int LO, int HI, typename F>
-cudaError_t with_depth(int d, F &&f)
+// f(std::integral_constant<int, d>{}, std::integral_constant<int, KIND>{}) for a runtime d in
+// [LO, HI]; with_sampler is its only caller.
+template <int LO, int HI, int KIND, typename F>
+cudaError_t with_depth(int d, F &f)
 {
     if constexpr (LO > HI)
         return cudaErrorInvalidValue;
+    else if (d == LO)
+        return f(std::integral_constant<int, LO>{}, std::integral_constant<int, KIND>{});
     else
-        return d == LO ? f(std::integral_constant<int, LO>{}) : with_depth<LO + 1, HI>(d, f);
+        return with_depth<LO + 1, HI, KIND>(d, f);
+}
+
+// f(D, KIND) with the compile-time depth and SamplerKind of the kernel that serves `c`, both as
+// std::integral_constant: the depths each exact sampler is instantiated for (v6 5..9, v5 1..10)
+// are listed here and nowhere else.
+template <typename F>
+cudaError_t with_sampler(const SamplerChoice &c, F &&f)
+{
+    switch (c.kind) {
+    case SAMPLER_PARALLEL: return with_depth<0, 0, SAMPLER_PARALLEL>(c.D, f);
+    case SAMPLER_SMALL: return with_depth<0, 0, SAMPLER_SMALL>(c.D, f);
+    case SAMPLER_V6: return with_depth<5, 9, SAMPLER_V6>(c.D, f);
+    default: return with_depth<1, 10, SAMPLER_V5>(c.D, f);
+    }
 }
 
 // ---------------------------------------------------------------------------
@@ -291,6 +310,146 @@ __device__ __forceinline__ void spec_descend(const double *val, int &node, doubl
 }
 
 // ---------------------------------------------------------------------------
+// pieces shared by the samplers
+// ---------------------------------------------------------------------------
+// The root's child the reference's descent visits first: the one holding the OLDER half of the
+// ring (collections/prioritized.py:255-258 with the bounds of :229-241).
+__device__ __forceinline__ int older_child(const SampleArgs &a, long long npop)
+{
+    return ((npop & (a.nslots - 1)) >= (a.nslots >> 1)) ? 3 : 2;
+}
+
+// The sum-tree and min-tree roots before the draws (priority_sums.sum(), priority_mins.min(),
+// :58-59) and the batch size, for the weights k_weights computes after the sample.
+__device__ __forceinline__ void record_roots(const SampleArgs &a, double total, double mroot)
+{
+    a.st->last_total = total;
+    a.st->last_min = mroot;
+    a.st->last_n = a.n;
+}
+
+// np.random.uniform(0.0, root) = 0.0 + (root - 0.0) * u (:302), then _find (:245-258) through
+// the T levels held in `top`: the root step into the older half first, spec_descend below it.
+// Returns the node at level T - 1; pos is left as the position inside it.  One warp.
+template <int T>
+__device__ __forceinline__ int descend_top(const double *top, int older, double u, double &pos,
+                                           int lane)
+{
+    pos = __dmul_rn(top[1], u);
+    int node = older;
+    const double left = top[older];
+    if (!(pos < left)) {
+        pos = __dsub_rn(pos, left);
+        node = older ^ 1;
+    }
+    spec_descend<T - 2>(top, node, pos, lane); // level 1 -> T-1
+    return node;
+}
+
+// The 2^(D+1) - 2 nodes of the D levels below heap node `node` into sub[2, 2^(D+1)), relative
+// heap order (node r has children 2r, 2r+1, leaves at r >= 2^D).  Each level's slice of the
+// subtree is contiguous in the heap, so the warp's lanes fetch it in ONE round trip: no load
+// waits for a store, and the compiler issues them ahead.  Written as one load and store per pair:
+// holding every pair in registers before the first store measured 0.4 % slower in v6 (H100 SXM,
+// 700 W), where it costs the 128-register main warp its allocation.  One warp; sub is readable by
+// the warp on return.
+template <int D>
+__device__ __forceinline__ void load_subtree(double *sub, const double *sum, unsigned node,
+                                             uint64_t pol, int lane)
+{
+    constexpr int PAIRS = (1 << D) - 1; // child pairs below `node`
+    constexpr int NIT = (PAIRS + 31) / 32;
+    const double2 *sum2 = reinterpret_cast<const double2 *>(sum);
+#pragma unroll
+    for (int it = 0; it < NIT; it++) {
+        int q = lane + 32 * it;
+        q = q < 1 ? 1 : (q > PAIRS ? PAIRS : q);
+        const int dq = 31 - __clz(q);
+        reinterpret_cast<double2 *>(sub)[q] =
+            ld_tree_pair(sum2 + ((node << dq) + (unsigned)(q - (1 << dq))), pol);
+    }
+    __syncwarp();
+}
+
+// Heap nodes [0, 2^T) -> top by cp.async.bulk, completing on `bar`.  One thread.  The proxy
+// fence makes earlier generic-proxy writes to the tree by this CTA (fused write-back) visible
+// to the bulk copy engine.
+template <int T>
+__device__ __forceinline__ void top_load_start(double *top, const double *sum, uint64_t *bar)
+{
+    constexpr int TOPN = 1 << T;
+    asm volatile("fence.proxy.async;" ::: "memory");
+    mbar_expect_tx(bar, TOPN * 8);
+#pragma unroll
+    for (int c = 0; c < 4; c++)
+        bulk_g2s(top + c * (TOPN / 4), sum + c * (TOPN / 4), TOPN * 2, bar);
+}
+
+// top -> heap nodes [0, 2^T) by a bulk store, once the whole CTA is done with it.  All threads
+// of the CTA; thread 0 returns when the store is complete.
+template <int T>
+__device__ __forceinline__ void top_store(double *sum, const double *top)
+{
+    constexpr int TOPN = 1 << T;
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int c = 0; c < 4; c++)
+            bulk_s2g(sum + c * (TOPN / 4), top + c * (TOPN / 4), TOPN * 2);
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    }
+}
+
+static constexpr int EX_RING = 64; // finished draws waiting for the publisher
+
+// One finished draw of an exact sampler: the ring slot of its leaf, the staged buffer its
+// subtree is in (v6's ascent warps; V6_NBUF = sub_own), its priority.
+struct DrawEnt {
+    int slot, buf;
+    double prio;
+};
+
+// Publisher warp of v5 and v6: as the deciding warp releases finished draws (*done = number
+// of draws in `ring`), stores their outputs 32 at a time, releases each chunk to the gather
+// CTAs (fused step) and its ring entries to the deciding warp (*pub), and finally writes the
+// weights normalised by the batch minimum.  roots = {total, min root}, stored by the deciding
+// warp before its first release.
+__device__ __forceinline__ void publish_draws(const SampleArgs &a, const DrawEnt *ring,
+                                              const int *done, int *pub, const double *roots,
+                                              long long npop)
+{
+    constexpr int CHUNK = 32;
+    const int lane = threadIdx.x & 31;
+    double total = 0.0, mroot = 0.0, bmin = INFINITY;
+    const double len = (double)(a.st->napp - npop);
+    for (int k0 = 0; k0 < a.n; k0 += CHUNK) {
+        const int kend = (a.n - k0 < CHUNK) ? a.n : k0 + CHUNK;
+        while (ld_acquire_smem(done) < kend) __nanosleep(200);
+        if (k0 == 0) {
+            total = roots[0];
+            mroot = roots[1];
+        }
+        const int k = k0 + lane;
+        if (k < kend)
+            store_draw(a, k, ring[k % EX_RING].slot, ring[k % EX_RING].prio, total, mroot, len,
+                       npop, bmin);
+        __syncwarp();
+        if (lane == 0) {
+            if (a.ready) st_release_gpu(a.ready, a.seq_base | (unsigned long long)kend);
+            st_release_smem(pub, kend);
+        }
+        __syncwarp();
+    }
+    if (a.weight && a.norm == B2RL_NORM_BATCH) {
+        // np.min(probabilities) over the batch, replay_buffers/prioritized.py:60
+        for (int o = 16; o > 0; o >>= 1) bmin = fmin(bmin, __shfl_xor_sync(0xffffffffu, bmin, o));
+        store_batch_weights(a, total, bmin, len, lane, 32);
+    }
+}
+
+// ---------------------------------------------------------------------------
 // EXACT sampler for deep trees (levels >= TOP_LEVELS).  Called by ALL threads
 // of the CTA (it uses __syncthreads); warps >= 4 only take part in the
 // barriers.
@@ -309,18 +468,16 @@ __device__ __forceinline__ void spec_descend(const double *val, int &node, doubl
 // (release/acquire on `main_done` + "node != previous node").  The arithmetic
 // of the main warp is the reference's, so indices stay bit-identical.
 // Shared memory: [top 2^14 f64][sub_own 2^(D+1)][sub_pref 3 x 2^(D+1)]
-// [o_prio ring][2 f64][o_slot ring][flags][mbarrier].
+// [DrawEnt ring][2 f64][flags][mbarrier].
 // ---------------------------------------------------------------------------
-static constexpr int EX_RING = 64;    // finished draws waiting for the publisher
 static constexpr int EX_NSCOUT = 2;
 static constexpr int EX_LAG = 2;
 static constexpr int EX_NBUF = EX_LAG + 1;
 
 constexpr size_t exact_deep_smem_bytes(int D)
 {
-    return sizeof(double) * ((size_t(1) << TOP_LEVELS) + (size_t(2) << D) * (1 + EX_NBUF) +
-                             EX_RING + 2) +
-           sizeof(int) * (EX_RING + 16) + 16;
+    return sizeof(double) * ((size_t(1) << TOP_LEVELS) + (size_t(2) << D) * (1 + EX_NBUF) + 2) +
+           sizeof(DrawEnt) * EX_RING + sizeof(int) * 16 + 16;
 }
 
 template <int D>
@@ -329,18 +486,15 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
     constexpr int T = TOP_LEVELS;
     constexpr int TOPN = 1 << T;
     constexpr int SUBN = 2 << D;
-    constexpr int PAIRS = (1 << D) - 1; // child pairs below the chosen top node
-    constexpr int NIT = (PAIRS + 31) / 32;
     constexpr int CHUNK = 32;
     constexpr int NSCOUT = EX_NSCOUT, LAG = EX_LAG, NBUF = EX_NBUF, RING = EX_RING;
     constexpr int F_READY = 0, F_NODE = 4, F_DONE = 8, F_PUB = 9;
     double *top = smem_d;
     double *sub_own = smem_d + TOPN;
-    double *sub_pref = sub_own + SUBN;              // [NBUF][SUBN]
-    double *o_prio = sub_pref + NBUF * SUBN;        // [RING]
-    double *s_stat = o_prio + RING;                 // total, min-root
-    int *o_slot = reinterpret_cast<int *>(s_stat + 2); // [RING]
-    int *flags = o_slot + RING; // ready_seq[NBUF] @0, pred_node[NBUF] @4, main_done @8, pub_done @9
+    double *sub_pref = sub_own + SUBN;                                   // [NBUF][SUBN]
+    DrawEnt *ring = reinterpret_cast<DrawEnt *>(sub_pref + NBUF * SUBN); // [RING]
+    double *s_stat = reinterpret_cast<double *>(ring + RING);           // total, min-root
+    int *flags = reinterpret_cast<int *>(s_stat + 2); // ready_seq[NBUF] @0, pred_node[NBUF] @4, main_done @8, pub_done @9
     uint64_t *bar = reinterpret_cast<uint64_t *>(flags + 16);
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
@@ -351,22 +505,14 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
         flags[F_PUB] = 0;
         mbar_init(bar, 1);
         mbar_fence_init();
-        // earlier generic-proxy writes to the tree by this CTA (fused write-back)
-        // must be visible to the bulk copy engine
-        asm volatile("fence.proxy.async;" ::: "memory");
-        mbar_expect_tx(bar, TOPN * 8);
-#pragma unroll
-        for (int c = 0; c < 4; c++)
-            bulk_g2s(top + c * (TOPN / 4), a.sum + c * (TOPN / 4), TOPN * 2, bar);
+        top_load_start<T>(top, a.sum, bar);
     }
     __syncthreads();
     if (warp < 4) mbar_wait(bar, 0);
 
-    const long long mask = a.nslots - 1;
     const long long npop = a.st->npop;
-    const int older = ((npop & mask) >= (a.nslots >> 1)) ? 3 : 2;
+    const int older = older_child(a, npop);
     const uint64_t pol = policy_evict_last();
-    const double2 *sum2 = reinterpret_cast<const double2 *>(a.sum);
 
     if (warp >= 1 && warp <= NSCOUT) {
         // ------------------------------ scouts -------------------------------
@@ -374,30 +520,9 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
             const double uk = a.u[k];
             // draws 0..k-1-LAG must be complete (their stores visible) before we read
             while (ld_acquire_smem(&flags[F_DONE]) < k - LAG) __nanosleep(64);
-            double pos = uk * top[1]; // approximate: up to LAG draws still in flight
-            int node = older;
-            {
-                const double left = top[older];
-                if (!(pos < left)) { pos -= left; node = older ^ 1; }
-            }
-            spec_descend<T - 2>(top, node, pos, lane);
-            double *dst = sub_pref + (k % NBUF) * SUBN;
-            const unsigned unode = (unsigned)node;
-            double2 tmp[NIT];
-#pragma unroll
-            for (int it = 0; it < NIT; it++) {
-                int q = lane + 32 * it;
-                q = q < 1 ? 1 : (q > PAIRS ? PAIRS : q);
-                const int dq = 31 - __clz(q);
-                tmp[it] = ld_tree_pair(sum2 + ((unode << dq) + (unsigned)(q - (1 << dq))), pol);
-            }
-#pragma unroll
-            for (int it = 0; it < NIT; it++) {
-                int q = lane + 32 * it;
-                q = q < 1 ? 1 : (q > PAIRS ? PAIRS : q);
-                reinterpret_cast<double2 *>(dst)[q] = tmp[it];
-            }
-            __syncwarp();
+            double pos; // approximate: up to LAG draws still in flight
+            const int node = descend_top<T>(top, older, uk, pos, lane);
+            load_subtree<D>(sub_pref + (k % NBUF) * SUBN, a.sum, (unsigned)node, pol, lane);
             if (lane == 0) {
                 flags[F_NODE + (k % NBUF)] = node;
                 st_release_smem(&flags[F_READY + (k % NBUF)], k);
@@ -407,11 +532,9 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
     } else if (warp == 0) {
         // ------------------------------- main --------------------------------
         if (lane == 0) {
-            const double total = top[1]; // priority_sums.sum(), :58
-            const double mroot = a.mn[1]; // priority_mins.min(), :59
-            a.st->last_total = total;
-            a.st->last_min = mroot;
-            a.st->last_n = a.n;
+            const double total = top[1];
+            const double mroot = a.mn[1];
+            record_roots(a, total, mroot);
             s_stat[0] = total;
             s_stat[1] = mroot;
         }
@@ -427,17 +550,8 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
             for (int kk = 0; kk < kend; kk++) {
                 const int k = k0 + kk;
                 const double uk = __shfl_sync(0xffffffffu, u_lane, kk);
-                // np.random.uniform(0.0, root) = 0.0 + (root - 0.0) * u, :302
-                double pos = __dmul_rn(top[1], uk);
-                int node = older;
-                {
-                    const double left = top[older];
-                    if (!(pos < left)) {
-                        pos = __dsub_rn(pos, left);
-                        node = older ^ 1;
-                    }
-                }
-                spec_descend<T - 2>(top, node, pos, lane); // level 1 -> T-1
+                double pos;
+                const int node = descend_top<T>(top, older, uk, pos, lane);
                 const unsigned unode = (unsigned)node;
                 // ---- the D levels under `node`: staged by the scout, or fetched here
                 const double *sub;
@@ -450,22 +564,7 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
                     sub = sub_pref + (k % NBUF) * SUBN;
                     hits++;
                 } else {
-                    double2 tmp[NIT];
-#pragma unroll
-                    for (int it = 0; it < NIT; it++) {
-                        int q = lane + 32 * it;
-                        q = q < 1 ? 1 : (q > PAIRS ? PAIRS : q);
-                        const int dq = 31 - __clz(q);
-                        tmp[it] =
-                            ld_tree_pair(sum2 + ((unode << dq) + (unsigned)(q - (1 << dq))), pol);
-                    }
-#pragma unroll
-                    for (int it = 0; it < NIT; it++) {
-                        int q = lane + 32 * it;
-                        q = q < 1 ? 1 : (q > PAIRS ? PAIRS : q);
-                        reinterpret_cast<double2 *>(sub_own)[q] = tmp[it];
-                    }
-                    __syncwarp();
+                    load_subtree<D>(sub_own, a.sum, unode, pol, lane);
                     sub = sub_own;
                 }
                 int rel = 1;
@@ -499,8 +598,8 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
                     if (lane == 0) top[node >> (j + 1)] = v;
                 }
                 if (lane == 0) {
-                    o_slot[k % RING] = (int)(leafnode - (unsigned)a.nslots);
-                    o_prio[k % RING] = prio;
+                    ring[k % RING].slot = (int)(leafnode - (unsigned)a.nslots);
+                    ring[k % RING].prio = prio;
                     // publish "draws 0..k are complete" (global + shared stores above)
                     st_release_smem(&flags[F_DONE], k + 1);
                 }
@@ -512,44 +611,10 @@ __device__ __forceinline__ void exact_deep(const SampleArgs &a, double *smem_d)
         }
         if (lane == 0) a.st->pad = hits | (late << 16); // scout diagnostics: hits, not-ready
     } else if (warp == 3) {
-        // ----------------------------- publisher -----------------------------
-        double total = 0.0, mroot = 0.0, bmin = INFINITY;
-        const double len = (double)(a.st->napp - npop);
-        for (int k0 = 0; k0 < a.n; k0 += CHUNK) {
-            const int kend = (a.n - k0 < CHUNK) ? a.n : k0 + CHUNK;
-            while (ld_acquire_smem(&flags[F_DONE]) < kend) __nanosleep(200);
-            if (k0 == 0) {
-                total = s_stat[0];
-                mroot = s_stat[1];
-            }
-            const int k = k0 + lane;
-            if (k < kend)
-                store_draw(a, k, o_slot[k % RING], o_prio[k % RING], total, mroot, len, npop,
-                           bmin);
-            __syncwarp();
-            if (lane == 0) {
-                if (a.ready) st_release_gpu(a.ready, a.seq_base | (unsigned long long)kend);
-                st_release_smem(&flags[F_PUB], kend);
-            }
-            __syncwarp();
-        }
-        if (a.weight && a.norm == B2RL_NORM_BATCH) {
-            // np.min(probabilities) over the batch, replay_buffers/prioritized.py:60
-            for (int o = 16; o > 0; o >>= 1) bmin = fmin(bmin, __shfl_xor_sync(0xffffffffu, bmin, o));
-            store_batch_weights(a, total, bmin, len, lane, 32);
-        }
+        publish_draws(a, ring, &flags[F_DONE], &flags[F_PUB], s_stat, npop);
     }
     __syncthreads();
-    // publish the shared-memory levels (zeroed state) back to HBM: bulk store
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int c = 0; c < 4; c++)
-            bulk_s2g(a.sum + c * (TOPN / 4), top + c * (TOPN / 4), TOPN * 2);
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    }
+    top_store<T>(a.sum, top); // the shared-memory levels (zeroed state) back to HBM
 }
 
 // ---------------------------------------------------------------------------
@@ -566,19 +631,12 @@ __device__ __forceinline__ void exact_small(const SampleArgs &a, double *smem_d)
 
     if (tid < 32) {
         const int lane = tid;
-        const long long mask = a.nslots - 1;
         const long long npop = a.st->npop;
-        // The reference's root visits its OLDER half first
-        // (collections/prioritized.py:255-258 with the bounds of :229-241).
-        const int older = ((npop & mask) >= (a.nslots >> 1)) ? 3 : 2;
-        const double total = top[1]; // priority_sums.sum(), :58
-        const double mroot = a.mn[1]; // priority_mins.min(), :59
+        const int older = older_child(a, npop);
+        const double total = top[1];
+        const double mroot = a.mn[1];
         const double len = (double)(a.st->napp - npop);
-        if (lane == 0) {
-            a.st->last_total = total;
-            a.st->last_min = mroot;
-            a.st->last_n = a.n;
-        }
+        if (lane == 0) record_roots(a, total, mroot);
         double bmin = INFINITY;
         double unext = a.n > 0 ? a.u[0] : 0.0;
         for (int k = 0; k < a.n; k++) {
@@ -634,12 +692,11 @@ __device__ __forceinline__ void exact_small(const SampleArgs &a, double *smem_d)
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ void sample_parallel(const SampleArgs &a, double *red)
 {
-    const long long mask = a.nslots - 1;
     const long long npop = a.st->npop;
     const double root = a.sum[1];
     const double mroot = a.mn[1];
     const double len = (double)(a.st->napp - npop);
-    const int older = ((npop & mask) >= (a.nslots >> 1)) ? 3 : 2;
+    const int older = older_child(a, npop);
     const double older_v = a.sum[older];
     double bmin = INFINITY;
     for (int k = threadIdx.x; k < a.n; k += blockDim.x) {
@@ -677,11 +734,7 @@ __device__ __forceinline__ void sample_parallel(const SampleArgs &a, double *red
         const double prio = a.sum[node];
         store_draw(a, k, node - a.nslots, prio, root, mroot, len, npop, bmin);
     }
-    if (threadIdx.x == 0) {
-        a.st->last_total = root;
-        a.st->last_min = mroot;
-        a.st->last_n = a.n;
-    }
+    if (threadIdx.x == 0) record_roots(a, root, mroot);
     if (a.weight && a.norm == B2RL_NORM_BATCH) {
         for (int o = 16; o > 0; o >>= 1) bmin = fmin(bmin, __shfl_xor_sync(0xffffffffu, bmin, o));
         if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = bmin;
@@ -1122,8 +1175,8 @@ __device__ __forceinline__ void tree_update_multi(const UpdateArgs &a, unsigned 
 //     a decision depends on stays within (n + 180) 2^-53 root and EPS =
 //     (n + 64) 2^-46 root is > 45x that for every n >= 1 (DESIGN.md has the budget).
 //     Any doubt (late or wrong scout, margin, conflict) -> SLOW PATH: wait until
-//     the exact tree has caught up and run the reference's arithmetic on it (the
-//     v5 code).  Never wrong, only slow; the count is reported
+//     the exact tree has caught up and run the reference's arithmetic on it (v5's
+//     descend_top, load_subtree, spec_descend).  Never wrong, only slow; the count is reported
 //     (b2rl_per_info.scout_hits: fast | slow << 16).
 //   * the ascent warps apply draw k to the EXACT tree (shared-memory top +
 //     global bottom) with the reference's bottom-up adds, a few draws behind;
@@ -1176,10 +1229,25 @@ __host__ __device__ constexpr size_t v6_buf_doubles(int D)
 
 constexpr size_t exact_v6_smem_bytes(int D)
 {
-    // etop, M, P_lo, P_hi(64) + rootA + stat(2) + pad, sub_own, NBUF x staged buffer, o_prio
+    // etop, M, P_lo, P_hi(64) + rootA + stat(2) + pad, sub_own, NBUF x staged buffer, ring
     return sizeof(double) * ((size_t(1) << V6_T) + 2 * V6_NTOP + 80 + (size_t(2) << D) +
-                             V6_NBUF * v6_buf_doubles(D) + 2 * EX_RING) +
-           sizeof(int) * 32 + sizeof(unsigned short) * V6_NTOP + 16 + 8 * V6_NBUF;
+                             V6_NBUF * v6_buf_doubles(D)) +
+           sizeof(DrawEnt) * EX_RING + sizeof(int) * 32 + sizeof(unsigned short) * V6_NTOP + 16 +
+           8 * V6_NBUF;
+}
+
+// Levels 11..0 of v6's exact top from level 12: the ascent warps keep level 12 exact, and every
+// node above it is fl(left + right) of its children.  Threads t0, t0 + nt, ... of the caller
+// share the work; barrier() is the caller's barrier over those threads, after each level.
+template <typename Barrier>
+__device__ __forceinline__ void v6_rebuild_top(double *etop, int t0, int nt, Barrier barrier)
+{
+    for (int lv = V6_T - 2; lv >= 0; lv--) {
+        const int wdt = 1 << lv;
+        for (int i = t0; i < wdt; i += nt)
+            etop[wdt + i] = __dadd_rn(etop[2 * (wdt + i)], etop[2 * (wdt + i) + 1]);
+        barrier();
+    }
 }
 
 // Dynamic shared memory of the sampler `c` serving the draw `a` (launch_sample in sampler.cu,
@@ -1206,8 +1274,6 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
     constexpr int BUFN = (int)v6_buf_doubles(D);
     // the leaf window: [32] lower bounds, [32] priorities, end, first leaf (relative to 2^D)
     constexpr int O_WLO = SUBN, O_WPR = SUBN + 32, O_WEND = SUBN + 64, O_WFIRST = SUBN + 65;
-    constexpr int PAIRS = (1 << D) - 1;         // child pairs of a whole subtree (slow path)
-    constexpr int NIT = (PAIRS + 31) / 32;
     constexpr int CHUNK = 32;
     constexpr int NSCOUT = V6_NSCOUT, LAG = V6_LAG, NBUF = V6_NBUF, RING = EX_RING;
     constexpr int NASC = V6_NASC;
@@ -1239,12 +1305,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
     unsigned long long *ready64 = reinterpret_cast<unsigned long long *>(s_misc + 8);
     double *sub_own = s_misc + 16;
     double *sub_pref = sub_own + SUBN;          // [NBUF][BUFN]
-    // one 16-byte entry per decided draw, read by the ascent warp and by the publisher:
-    // {ring slot of the leaf, staged buffer (NBUF = sub_own), priority}
-    struct DrawEnt {
-        int slot, buf;
-        double prio;
-    };
+    // one entry per decided draw, read by the ascent warp and by the publisher
     DrawEnt *ring = reinterpret_cast<DrawEnt *>(sub_pref + NBUF * BUFN); // [RING]
     int *flags = reinterpret_cast<int *>(ring + RING);                   // [32]
     uint64_t *bar = reinterpret_cast<uint64_t *>(flags + 32); // [1 + NBUF]: top copy, staged buffers
@@ -1270,18 +1331,13 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
         mbar_init(bar, 1);
         for (int i = 0; i < NBUF; i++) mbar_init(bar + 2 + i, 1);
         mbar_fence_init();
-        asm volatile("fence.proxy.async;" ::: "memory");
-        mbar_expect_tx(bar, TOPN * 8);
-#pragma unroll
-        for (int c = 0; c < 4; c++)
-            bulk_g2s(etop + c * (TOPN / 4), a.sum + c * (TOPN / 4), TOPN * 2, bar);
+        top_load_start<T>(etop, a.sum, bar);
     }
     __syncthreads();
     mbar_wait(bar, 0);
 
-    const long long mask = a.nslots - 1;
     const long long npop = a.st->npop;
-    const int older = ((npop & mask) >= (a.nslots >> 1)) ? 3 : 2;
+    const int older = older_child(a, npop);
     const int oflip = older == 2 ? 0 : NTOP / 2; // descent order o <-> node 4096 + (o ^ oflip)
     // ---- the approximate tables, from the exact top
     for (int o = threadIdx.x; o < NTOP; o += blockDim.x) {
@@ -1307,7 +1363,6 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
     __syncthreads();
 
     const uint64_t pol = policy_evict_last();
-    const double2 *sum2 = reinterpret_cast<const double2 *>(a.sum);
     const double root0 = etop[1];
     if (threadIdx.x == 0) s_misc[0] = root0;
     // decision margin (see the header comment / DESIGN.md)
@@ -1408,10 +1463,8 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
     } else if (warp == V6_W_MAIN) {
         // ------------------------------- main --------------------------------
         if (lane == 0) {
-            const double mroot = a.mn[1]; // priority_mins.min(), :59
-            a.st->last_total = root0;     // priority_sums.sum(), :58
-            a.st->last_min = mroot;
-            a.st->last_n = a.n;
+            const double mroot = a.mn[1];
+            record_roots(a, root0, mroot);
             s_misc[1] = root0;
             s_misc[2] = mroot;
         }
@@ -1527,33 +1580,10 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                     nslow++;
                     while (asc_fenced() < k) {
                     }
-                    // the ascent warp keeps level 12 exact; levels 11..0 = fl(left + right)
-                    for (int lv = T - 2; lv >= 0; lv--) {
-                        const int wdt = 1 << lv;
-                        for (int i = lane; i < wdt; i += 32)
-                            etop[wdt + i] = __dadd_rn(etop[2 * (wdt + i)], etop[2 * (wdt + i) + 1]);
-                        __syncwarp();
-                    }
-                    double pos = __dmul_rn(etop[1], uk); // np.random.uniform(0.0, root), :302
-                    node = older;
-                    {
-                        const double left = etop[older];
-                        if (!(pos < left)) {
-                            pos = __dsub_rn(pos, left);
-                            node = older ^ 1;
-                        }
-                    }
-                    spec_descend<T - 2>(etop, node, pos, lane); // level 1 -> 12
-                    const unsigned unode = (unsigned)node;
-#pragma unroll
-                    for (int it = 0; it < NIT; it++) {
-                        int q = lane + 32 * it;
-                        q = q < 1 ? 1 : (q > PAIRS ? PAIRS : q);
-                        const int dq = 31 - __clz(q);
-                        reinterpret_cast<double2 *>(sub_own)[q] =
-                            ld_tree_pair(sum2 + ((unode << dq) + (unsigned)(q - (1 << dq))), pol);
-                    }
-                    __syncwarp();
+                    v6_rebuild_top(etop, lane, 32, [] { __syncwarp(); });
+                    double pos;
+                    node = descend_top<T>(etop, older, uk, pos, lane);
+                    load_subtree<D>(sub_own, a.sum, (unsigned)node, pol, lane);
                     rel = 1;
                     spec_descend<D>(sub_own, rel, pos, lane);
                     prio = sub_own[rel];
@@ -1681,51 +1711,13 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             atomicAdd(reinterpret_cast<unsigned long long *>(&s_misc[4]), (unsigned long long)c_awork);
         }
     } else if (warp == V6_W_PUB) {
-        // ----------------------------- publisher -----------------------------
-        double total = 0.0, mroot = 0.0, bmin = INFINITY;
-        const double len = (double)(a.st->napp - npop);
-        for (int k0 = 0; k0 < a.n; k0 += CHUNK) {
-            const int kend = (a.n - k0 < CHUNK) ? a.n : k0 + CHUNK;
-            while (ld_acquire_smem(&flags[F_MAIN]) < kend) __nanosleep(200);
-            if (k0 == 0) {
-                total = s_misc[1];
-                mroot = s_misc[2];
-            }
-            const int k = k0 + lane;
-            if (k < kend)
-                store_draw(a, k, ring[k % RING].slot, ring[k % RING].prio, total, mroot, len,
-                           npop, bmin);
-            __syncwarp();
-            if (lane == 0) {
-                if (a.ready) st_release_gpu(a.ready, a.seq_base | (unsigned long long)kend);
-                st_release_smem(&flags[F_PUB], kend);
-            }
-            __syncwarp();
-        }
-        if (a.weight && a.norm == B2RL_NORM_BATCH) {
-            for (int o = 16; o > 0; o >>= 1) bmin = fmin(bmin, __shfl_xor_sync(0xffffffffu, bmin, o));
-            store_batch_weights(a, total, bmin, len, lane, 32);
-        }
+        publish_draws(a, ring, &flags[F_MAIN], &flags[F_PUB], s_misc + 1, npop);
     }
     __syncthreads();
     if (a.dbg_cycles && threadIdx.x == 0) { // summed over the ascent warps: cycles per draw / B
         a.dbg_cycles[16] = *reinterpret_cast<const long long *>(&s_misc[3]);
         a.dbg_cycles[17] = *reinterpret_cast<const long long *>(&s_misc[4]);
     }
-    // levels 11..0 of the exact top from level 12 (see the ascent warp)
-    for (int lv = T - 2; lv >= 0; lv--) {
-        const int wdt = 1 << lv;
-        for (int i = threadIdx.x; i < wdt; i += blockDim.x)
-            etop[wdt + i] = __dadd_rn(etop[2 * (wdt + i)], etop[2 * (wdt + i) + 1]);
-        __syncthreads();
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int c = 0; c < 4; c++)
-            bulk_s2g(a.sum + c * (TOPN / 4), etop + c * (TOPN / 4), TOPN * 2);
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    }
+    v6_rebuild_top(etop, threadIdx.x, blockDim.x, [] { __syncthreads(); }); // see the ascent warp
+    top_store<T>(a.sum, etop);
 }
