@@ -555,6 +555,30 @@ int b2rl_trpo_line_search(int32_t n_cand, const float *cand, const float *gain0,
                           void *stream);
 
 /* ------------------------------------------------------------------------
+ * ACER's discrete-action loss gradient on one sequence of T steps
+ * (pfrl/agents/acer.py:16-115, 207-248, 423-552): fp32 storage, fp64
+ * accumulation, device pointers, one CTA.
+ * z, q [T, K]: the policy's Categorical._param (normalised logits) and the Q
+ * values.  avg_z [T, K]: the average model's logits (NULL without the trust
+ * region).  mu_z [T, K]: the behaviour policy's logits, or NULL for the online
+ * update (rho = 1).  actions int64 [T], rewards fp64 [T].  bootstrap: the
+ * device fp32 value of the state after the last step, or NULL for a terminal
+ * (R = 0).  truncate = 0 means truncation_threshold None; the threshold may be
+ * 0 or inf.  average_kl (fp64 [1], read and written) takes each step's
+ * KL(avg || pi) in reversed step order when use_trust_region is set.
+ * Writes g_z = d total / d z and g_q = d total / d q [T, K].  scratch: 10
+ * doubles per step. */
+int b2rl_acer_loss(int32_t T, int32_t K, const float *z, const float *q,
+                   const float *avg_z, const float *mu_z, const int64_t *actions,
+                   const double *rewards, const float *bootstrap, double gamma,
+                   int32_t truncate, double truncation_threshold,
+                   int32_t use_trust_region, double delta, double beta,
+                   double pi_loss_coef, double q_loss_coef,
+                   int32_t normalize_by_steps, int32_t use_q_opc,
+                   double *average_kl, double average_kl_decay, double *scratch,
+                   float *g_z, float *g_q, void *stream);
+
+/* ------------------------------------------------------------------------
  * SAC / TD3 / DDPG update tail (fp32, device pointers).
  * ---------------------------------------------------------------------- */
 

@@ -98,6 +98,22 @@ class AttributeSavingMixin(object):
             value.load_state_dict(torch.load(os.path.join(dirname, name + ".pt"), where))
 
 
+class AsyncAgent(Agent, metaclass=ABCMeta):
+    """Agent whose training is shared between processes (pfrl/agent.py:140-154)."""
+
+    @property
+    @abstractmethod
+    def process_idx(self):
+        """Index of the process, 0 for the representative one; None if not assigned."""
+        pass
+
+    @property
+    @abstractmethod
+    def shared_attributes(self):
+        """Names of the attributes the processes share."""
+        pass
+
+
 class BatchAgent(Agent, metaclass=ABCMeta):
     """Agent that steps a batch of environments; the single-env calls are
     the batch calls with a batch of one (pfrl/agent.py:157-200)."""

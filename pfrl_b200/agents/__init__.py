@@ -13,3 +13,4 @@ from pfrl_b200.agents.soft_actor_critic import SoftActorCritic  # NOQA
 from pfrl_b200.agents.td3 import DDPG, TD3  # NOQA
 from pfrl_b200.agents import ddpg  # NOQA  (module path of the reference)
 from pfrl_b200.agents.trpo import TRPO  # NOQA
+from pfrl_b200.agents.acer import ACER  # NOQA

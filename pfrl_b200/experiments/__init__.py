@@ -8,8 +8,4 @@ from pfrl_b200.experiments.evaluator import batch_run_evaluation_episodes  # NOQ
 from pfrl_b200.experiments.evaluator import run_evaluation_episodes  # NOQA
 from pfrl_b200.experiments import evaluation_hooks  # NOQA
 from pfrl_b200.experiments.evaluation_hooks import EvaluationHook  # NOQA
-
-
-def train_agent_async(*args, **kwargs):
-    """Asynchronous (A3C-style, multi-process) training is outside the rebuilt path."""
-    raise NotImplementedError("train_agent_async is out of scope of pfrl_b200")
+from pfrl_b200.experiments.train_agent_async import train_agent_async  # NOQA

@@ -17,7 +17,13 @@ observations and records live in the part ring and record store of
     by any live episode or any uncommitted current episode;
   * a recurrent-state ring in HBM: ``recurrent_state`` / ``next_recurrent_state``
     of every transition (device tensors, numpy arrays or None; any nesting of
-    tuples) flattened to one fp32 row each, at row ``absolute index % capacity``.
+    tuples) flattened to one fp32 row each, at row ``absolute index % capacity``;
+  * a behaviour-policy ring in HBM for ACER: the ``mu`` distribution appended with a
+    transition, as one fp32 row at the same row index (a ``Categorical``'s normalised
+    logits [K], or an ``Independent(Normal, 1)``'s loc and scale [2A]).  The first
+    ``mu`` fixes the layout.  The host episode table also records which episodes
+    ended on a terminal, so a sampled subsequence's last transition is known to be
+    terminal or not without reading the device.
 
 ``sample_episodes`` returns ``DeviceEpisodes``; ``batch_recurrent_experiences``
 turns it into the packed minibatch with one kernel launch
@@ -69,11 +75,14 @@ class DeviceEpisodes(collections.abc.Sequence):
     """The result of ``EpisodicReplayBuffer.sample_episodes``: n (sub)episodes
     that still live in HBM, described by absolute record ranges."""
 
-    def __init__(self, buffer, first, length, end):
+    def __init__(self, buffer, first, length, end, last_terminal=None):
         self.buffer = buffer
         self.first = np.asarray(first, dtype=np.int64)    # absolute record index
         self.length = np.asarray(length, dtype=np.int32)
         self.end = np.asarray(end, dtype=np.int64)        # one past the episode's last record
+        # whether each (sub)episode's last transition is terminal (host)
+        self.last_terminal = (np.zeros(len(self.length), dtype=bool) if last_terminal is None
+                              else np.asarray(last_terminal, dtype=bool))
         self._lists = None
 
     def __len__(self):
@@ -84,7 +93,7 @@ class DeviceEpisodes(collections.abc.Sequence):
         reverse=True)`` does to the materialised lists."""
         order = np.argsort(-self.length, kind="stable")
         return DeviceEpisodes(self.buffer, self.first[order], self.length[order],
-                              self.end[order])
+                              self.end[order], self.last_terminal[order])
 
     def batch(self, gamma, phi, device=None):
         """Device-side batch_recurrent_experiences (pfrl/replay_buffer.py:219-287)."""
@@ -123,6 +132,12 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
         self._rs_present = None                # [alloc, 2] uint8 (HBM)
         self._rs_present_host = None           # host mirror of _rs_present
         self._pend_rs = []                     # (ring row * 2 + side, flat row or None)
+        self._current_mu = collections.defaultdict(list)  # env_id -> [mu row or None]
+        self._terminal_ends = set()            # abs end of the live episodes ending terminal
+        self._mu_layout = None                 # (distribution class, width) of the first mu
+        self._mu_ring = None                   # [alloc, width] fp32 (HBM)
+        self._mu_present_host = None           # [alloc] bool
+        self._pend_mu = []                     # (ring row, mu row or None)
 
     # -- reference API ------------------------------------------------------
     def __len__(self):
@@ -146,11 +161,13 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
         rs = self._flat_state(kwargs.get("recurrent_state"))
         nrs = self._flat_state(kwargs.get("next_recurrent_state"))
         self.current_episode[env_id].append((rec, rs, nrs))
+        self._current_mu[env_id].append(self._flat_mu(kwargs.get("mu")))
         if is_state_terminal:
             self.stop_current_episode(env_id=env_id)
 
     def stop_current_episode(self, env_id=0):
         episode = self.current_episode.pop(env_id, None)
+        mus = self._current_mu.pop(env_id, None)
         if not episode:
             return
         L = len(episode)
@@ -159,7 +176,9 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
             # drop whole oldest episodes first: afterwards the live records are the
             # last <= capacity records of the store, which keeps exactly those
             while len(self._episodes) and self._n_live + L > cap:
-                self._n_live -= self._episodes.popleft()[1]
+                f, L_old, _ = self._episodes.popleft()
+                self._n_live -= L_old
+                self._terminal_ends.discard(f + L_old)
             if L > cap:
                 return  # longer than the whole buffer: the reference drops it too
         elif self._n_total + L > self._alloc_capacity:
@@ -173,10 +192,14 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
             if rs is not None or nrs is not None or self._rs_struct is not None:
                 self._pend_rs.append((row * 2, rs))
                 self._pend_rs.append((row * 2 + 1, nrs))
+            if self._mu_layout is not None:
+                self._pend_mu.append((row, mus[j]))
         self._n_total += L
         self._n_live += L
         seq = min(rec[5] for rec, _, _ in episode)
         self._episodes.append((first, L, seq))
+        if episode[-1][0][4]:
+            self._terminal_ends.add(first + L)
         while self._min_seq and self._min_seq[-1][1] >= seq:
             self._min_seq.pop()
         self._min_seq.append((self._ep_count, seq))
@@ -201,7 +224,7 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
         order, like random_subseq)."""
         assert len(self._episodes) >= n_episodes
         picked = [self._episodes[i] for i in sample_n_k(len(self._episodes), n_episodes)]
-        first, length, end = [], [], []
+        first, length, end, term = [], [], [], []
         for f, L, _ in picked:
             start, n = f, L
             if max_len is not None and L > max_len:
@@ -210,7 +233,8 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
             first.append(start)
             length.append(n)
             end.append(f + L)
-        return DeviceEpisodes(self, first, length, end)
+            term.append(start + n == f + L and f + L in self._terminal_ends)
+        return DeviceEpisodes(self, first, length, end, term)
 
     def save(self, filename):
         """Own format: the pickled live episodes in the reference's transition dicts, with
@@ -306,6 +330,71 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
             idx = torch.as_tensor(np.array([k for k, _ in have], dtype=np.int64)).to(dev)
             self._rs_ring.view(-1, self._rs_width).index_copy_(0, idx, rows)
 
+    # -- behaviour policies (ACER's mu) -------------------------------------------
+    def _flat_mu(self, mu):
+        """One fp32 row of ``mu`` (a device or host tensor; no copy to the host)."""
+        if mu is None:
+            return None
+        D = torch.distributions
+        if type(mu) is D.Categorical:
+            row = mu.logits.detach().reshape(-1)
+        elif (type(mu) is D.Independent and type(mu.base_dist) is D.Normal
+              and mu.reinterpreted_batch_ndims == 1):
+            row = torch.cat([mu.base_dist.loc.detach().reshape(-1),
+                             mu.base_dist.scale.detach().reshape(-1)])
+        else:
+            raise NotImplementedError(
+                "EpisodicReplayBuffer stores mu as a Categorical or an Independent(Normal, 1) "
+                "distribution, got %s" % type(mu).__name__)
+        layout = (type(mu), int(row.numel()))
+        if self._mu_layout is None:
+            self._mu_layout = layout
+        assert layout == self._mu_layout, \
+            "mu layout changed: %s of width %d, the buffer holds %s of width %d" % (
+                layout[0].__name__, layout[1], self._mu_layout[0].__name__, self._mu_layout[1])
+        return row.float() if row.dtype != torch.float32 else row
+
+    def _flush_mu(self):
+        pend = self._pend_mu
+        if not pend:
+            return
+        self._pend_mu = []
+        dev = self.device
+        if self._mu_ring is None:
+            self._mu_ring = torch.zeros((self._alloc_capacity, self._mu_layout[1]),
+                                        dtype=torch.float32, device=dev)
+            self._mu_present_host = np.zeros(self._alloc_capacity, dtype=bool)
+        # only the last write of a ring row may reach the scatter
+        pend = list({k: (k, r) for k, r in pend}.values())
+        self._mu_present_host[[k for k, _ in pend]] = [r is not None for _, r in pend]
+        have = [(k, r) for k, r in pend if r is not None]
+        if have:
+            rows = torch.stack([r if r.device == dev else r.to(dev) for _, r in have])
+            idx = torch.as_tensor(np.array([k for k, _ in have], dtype=np.int64))
+            self._mu_ring.index_copy_(0, idx.to(dev, non_blocking=True), rows)
+
+    def _mu_distribution(self, row):
+        """``row`` [width] rebuilt as the stored class with a batch axis of 1."""
+        cls, width = self._mu_layout
+        if cls is torch.distributions.Categorical:
+            return cls(logits=row[None])
+        A = width // 2
+        return torch.distributions.Independent(
+            torch.distributions.Normal(loc=row[None, :A], scale=row[None, A:]), 1)
+
+    def mu_rows(self, eps):
+        """The [T, width] mu rows of the one subsequence in ``eps``, on the device (a run
+        of consecutive ring rows, so a slice or two; no synchronisation)."""
+        assert len(eps) == 1 and self._mu_layout is not None
+        self._flush()
+        cap = self._alloc_capacity
+        r0, T = int(eps.first[0]) % cap, int(eps.length[0])
+        assert self._mu_present_host[(r0 + np.arange(T)) % cap].all(), \
+            "a sampled transition was appended without mu"
+        if r0 + T <= cap:
+            return self._mu_ring[r0:r0 + T]
+        return torch.cat([self._mu_ring[r0:], self._mu_ring[:r0 + T - cap]])
+
     # -- internals ----------------------------------------------------------
     def _oldest_live_part(self):
         seqs = []
@@ -328,6 +417,7 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
                 % self._part_capacity)
         DeviceNStepBuffer._flush(self)  # _live_min_seq stays empty: no second check there
         self._flush_states()
+        self._flush_mu()
 
     def _logical(self, eps):
         npop = self._n_total - min(self._n_total, self._alloc_capacity)
@@ -411,6 +501,13 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
         # every transition's own states, as the reference stores them
         absolute = np.concatenate([np.arange(f, f + L) for f, L in zip(srt.first, srt.length)])
         states = self._host_states(absolute)
+        mus = None
+        if self._mu_ring is not None:
+            rows = absolute % self._alloc_capacity
+            mu_rows = self._mu_ring[torch.as_tensor(rows).to(self.device)]
+            present = self._mu_present_host[rows]
+            mus = [self._mu_distribution(mu_rows[i]) if present[i] else None
+                   for i in range(len(rows))]
         Lmax = int(srt.length[0]) if len(srt) else 0
         row0 = np.concatenate([[0], np.cumsum([(srt.length > t).sum() for t in range(Lmax)])])
         lists = [None] * len(srt)
@@ -422,27 +519,39 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
                 k += 1
                 r = int(row0[t]) + j
                 a = ac[r]
-                ep.append(dict(state=st[r], action=a.item() if a.shape == () else a,
-                               reward=rw[j][t], next_state=ns[r], next_action=None,
-                               is_state_terminal=bool(tm[r]),
-                               recurrent_state=rs, next_recurrent_state=nrs))
+                tr = dict(state=st[r], action=a.item() if a.shape == () else a,
+                          reward=rw[j][t], next_state=ns[r], next_action=None,
+                          is_state_terminal=bool(tm[r]),
+                          recurrent_state=rs, next_recurrent_state=nrs)
+                if mus is not None and mus[k - 1] is not None:
+                    tr["mu"] = mus[k - 1]
+                ep.append(tr)
             lists[order[j]] = ep
         return lists
 
     def _rewards_f64(self, eps):
         """The stored fp64 rewards (the packed batch carries them rounded to fp32)."""
-        from pfrl_b200.replay_buffers.device_buffer import DeviceExperiences
-
-        first, _ = self._logical(eps)
-        idx = np.concatenate([np.arange(f, f + L) for f, L in zip(first, eps.length)])
-        ex = DeviceExperiences(self, len(idx), index=torch.as_tensor(idx).to(self.device))
-        out = self._gather(ex, 1.0, None, raw=True, want_steps=True)
-        sr = out["step_rewards"].cpu().numpy()[:, 0].tolist()
+        sr = self._rewards_f64_device(eps).cpu().numpy().tolist()
         res, k = [], 0
         for L in eps.length:
             res.append(sr[k:k + int(L)])
             k += int(L)
         return res
+
+    def _rewards_f64_device(self, eps):
+        """The stored fp64 rewards of ``eps``'s records, concatenated, on the device (the
+        indices go up with a non-blocking copy from page-locked memory)."""
+        from pfrl_b200.replay_buffers.device_buffer import DeviceExperiences
+
+        self._flush()
+        first, _ = self._logical(eps)
+        idx = np.concatenate([np.arange(f, f + L) for f, L in zip(first, eps.length)])
+        index = torch.from_numpy(idx)
+        if self.device.type == "cuda":
+            index = index.pin_memory()
+        ex = DeviceExperiences(self, len(idx), index=index.to(self.device, non_blocking=True))
+        out = self._gather(ex, 1.0, None, raw=True, want_steps=True)
+        return out["step_rewards"][:, 0]
 
     def _host_states(self, absolute):
         """(recurrent_state, next_recurrent_state) of the records with the given absolute

@@ -12,7 +12,7 @@ test files unmodified from where they lie.
     python tools/run_reference_tests.py experiments_tests/test_evaluator.py -k batch
 
 Files that test subsystems outside the rebuilt path (async training, persistent
-buffers, ACER/..., ALE wrappers) are not in the list.
+buffers, ALE wrappers, ...) are not in the list.
 """
 import os
 import subprocess
@@ -49,6 +49,12 @@ DEFAULT = [
     "utils_tests/test_conjugate_gradient.py",
     "nn_tests/test_recurrent_sequential.py", "nn_tests/test_recurrent_branched.py",
     "utils_tests/test_recurrent.py",
+    # ACER's function-level tests; _TestACER needs train_agent_async
+    "agents_tests/test_acer.py::TestDegenerateDistribution",
+    "agents_tests/test_acer.py::test_bias_correction_gaussian",
+    "agents_tests/test_acer.py::test_bias_correction_softmax",
+    "agents_tests/test_acer.py::test_compute_loss_with_kl_constraint_gaussian",
+    "agents_tests/test_acer.py::test_compute_loss_with_kl_constraint_softmax",
 ]
 
 PLUGIN = '''
