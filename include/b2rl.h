@@ -579,6 +579,23 @@ int b2rl_acer_loss(int32_t T, int32_t K, const float *z, const float *q,
                    float *g_z, float *g_q, void *stream);
 
 /* ------------------------------------------------------------------------
+ * REINFORCE's loss gradient over the N recorded steps of an update
+ * (pfrl/agents/reinforce.py:176-195): loss = sum_rows(-R log pi(a) - beta H)
+ * / batchsize.  fp32 storage, fp64 arithmetic, device pointers, one warp per
+ * row.  A Categorical gives z [N, D] (Categorical._param, normalised logits),
+ * int64 actions [N] and g_z [N, D]; loc and action_values are then NULL.  An
+ * Independent(Normal, 1) gives loc [N, D], scale [N, D] (NULL = 1), the
+ * sampled fp32 action_values [N, D] and g_loc [N, D]; g_scale [N, D] is
+ * written unless NULL; z is then NULL.  returns fp32 [N].  row_loss and
+ * row_entropy [N] (optional) take each row's loss term and entropy. */
+int b2rl_reinforce_loss(int64_t N, int32_t D, const float *z, const float *loc,
+                        const float *scale, const int64_t *actions,
+                        const float *action_values, const float *returns,
+                        int32_t batchsize, double beta, float *g_z, float *g_loc,
+                        float *g_scale, float *row_loss, float *row_entropy,
+                        void *stream);
+
+/* ------------------------------------------------------------------------
  * SAC / TD3 / DDPG update tail (fp32, device pointers).
  * ---------------------------------------------------------------------- */
 

@@ -14,3 +14,4 @@ from pfrl_b200.agents.td3 import DDPG, TD3  # NOQA
 from pfrl_b200.agents import ddpg  # NOQA  (module path of the reference)
 from pfrl_b200.agents.trpo import TRPO  # NOQA
 from pfrl_b200.agents.acer import ACER  # NOQA
+from pfrl_b200.agents.reinforce import REINFORCE  # NOQA

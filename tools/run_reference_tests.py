@@ -55,6 +55,7 @@ DEFAULT = [
     "agents_tests/test_acer.py::test_bias_correction_softmax",
     "agents_tests/test_acer.py::test_compute_loss_with_kl_constraint_gaussian",
     "agents_tests/test_acer.py::test_compute_loss_with_kl_constraint_softmax",
+    "agents_tests/test_reinforce.py",
 ]
 
 PLUGIN = '''
