@@ -1471,34 +1471,48 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
         // The loop is software-pipelined around one measured fact: a shared-memory LOAD
         // issued behind this warp's own STOREs waits 100-200 cycles for them to drain
         // (ncu: three such load -> DADD pairs were 45 % of the draw).  So every draw issues
-        // ALL its loads first -- including the ones the NEXT draw needs -- and its stores
-        // last.  The next draw's table entries are therefore read before this draw's update
-        // is stored; the one missing update is applied in registers (ord_prev, p_prev).
+        // ALL its loads first and its stores last, and the loads include what the next two
+        // draws need: draw k reads the table entries and the window of draw k + 1 (at the
+        // ready word it read during draw k - 1) and the ready word of draw k + 2.  So the
+        // first shared-memory access after a draw's stores is never a load the next decision
+        // waits for (reading the next draw's ready word there, and everything it addresses
+        // behind it, cost 146 of the 743 cycles of a draw).  The next draw's table entries
+        // are read before this draw's update is stored; the one missing update is applied
+        // in registers (ord_prev, p_prev).
         double rootA = root0;
         int nfast = 0, nslow = 0;
-        // prefetched state of the draw about to be decided
+        // prefetched state of the draw about to be decided; its prefix stays in two parts,
+        // added in the decision, so that no instruction before the stores waits for the loads
         int pf_rs = -1, pf_o = 0, pf_seen = 0, pf_last = 0;
-        double pf_pre = 0.0, pf_mass = 0.0;
+        double pf_phi = 0.0, pf_plo = 0.0, pf_mass = 0.0;
         double pf_wlo = 0.0, pf_wpr = 0.0, pf_wend = 0.0; // the leaf window, one leaf per lane
         int pf_wfirst = 0;
         bool pf_stale = false;      // read before the previous draw's stores
         int ord_prev = -1;
         double p_prev = 0.0;
         long long c_ready = 0, c_decide = 0, c_queue = 0, c_loads = 0, c_stores = 0;
-        auto prefetch = [&](int k) {
-            const int b = k % NBUF;
-            // plain (volatile) load of the ready word: an acquire would park this warp until
-            // the load returns; the loads below are performed after it in the SM's in-order
-            // shared-memory pipe, behind the scout's release, which is all the ordering needed
+        // c_late / n_late: draws whose staging was not released when its ready word was read
+        // (spin and reload); c_pref: issuing the prefetch of the next draw
+        long long c_late = 0, n_late = 0, c_pref = 0;
+        // plain (volatile) load of a draw's ready word: an acquire would park this warp until
+        // the load returns; the loads of prefetch_from are performed after it in the SM's
+        // in-order shared-memory pipe, behind the scout's release, which is all the ordering
+        // needed
+        auto ready_word = [&](int k) {
             unsigned long long wv;
             asm volatile("ld.volatile.shared.b64 %0, [%1];"
                          : "=l"(wv)
-                         : "r"(smem_u32(&ready64[b]))
+                         : "r"(smem_u32(&ready64[k % NBUF]))
                          : "memory");
+            return wv;
+        };
+        auto prefetch_from = [&](int k, unsigned long long wv) {
+            const int b = k % NBUF;
             pf_rs = (int)(wv >> 32);
             pf_o = (int)(wv & (NTOP - 1));          // garbage unless pf_rs == k, but in range
             pf_seen = (int)((wv >> 12) & 0xfffffu);
-            pf_pre = phi[pf_o >> 6] + plo[pf_o];
+            pf_phi = phi[pf_o >> 6];
+            pf_plo = plo[pf_o];
             pf_mass = mtab[pf_o];
             pf_last = lastd[pf_o];
             const double *w = sub_pref + b * BUFN;
@@ -1507,7 +1521,9 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             pf_wend = w[O_WEND];
             pf_wfirst = *reinterpret_cast<const int *>(&w[O_WFIRST]);
         };
-        if (a.n > 0) prefetch(0);
+        unsigned long long nx_wv = 0; // the ready word of the draw after the prefetched one
+        if (a.n > 0) prefetch_from(0, ready_word(0));
+        if (a.n > 1) nx_wv = ready_word(1);
         for (int k0 = 0; k0 < a.n; k0 += CHUNK) {
             const double u_lane = (k0 + lane < a.n) ? a.u[k0 + lane] : 0.0;
             const int kend = (a.n - k0 < CHUNK) ? a.n - k0 : CHUNK;
@@ -1522,6 +1538,7 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                 bool fast = false;
                 // ---- the scout's staging of draw k: prefetched, or wait for it (bounded)
                 if (pf_rs != k) {
+                    const long long tl0 = V6_CLK();
                     for (int spin = 0; spin < 48; spin++) {
                         unsigned long long wv;
                         asm volatile("ld.acquire.cta.shared.b64 %0, [%1];"
@@ -1530,46 +1547,37 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                                      : "memory");
                         if ((int)(wv >> 32) == k) break;
                     }
-                    prefetch(k);
+                    prefetch_from(k, ready_word(k));
                     pf_stale = false;
-                }
-                // this draw's prefetched state moves to locals; the NEXT draw's loads start now,
-                // behind no store of this warp, and overlap the whole decision below
-                const int c_rs = pf_rs, c_o = pf_o, c_seen = pf_seen, c_last = pf_last;
-                const double c_pre = pf_pre, c_mass = pf_mass;
-                const double c_wlo = pf_wlo, c_wpr = pf_wpr, c_wend = pf_wend;
-                const int c_wfirst = pf_wfirst;
-                const bool c_stale = pf_stale;
-                if (k + 1 < a.n) {
-                    prefetch(k + 1);
-                    pf_stale = true;
+                    c_late += V6_CLK() - tl0;
+                    n_late++;
                 }
                 const long long tm1 = V6_CLK();
-                if (c_rs == k && !(a.dbg_slow_every > 0 && k % a.dbg_slow_every == 0)) {
-                    const int o = c_o;
+                if (pf_rs == k && !(a.dbg_slow_every > 0 && k % a.dbg_slow_every == 0)) {
+                    const int o = pf_o;
                     // a draw not yet applied to the exact tree when the copy was taken chose
                     // the same node?  (draw j is recorded as j + 1; the previous draw may
                     // still be missing from the table when the entry was read)
-                    const bool conflict = c_last > c_seen || (c_stale && ord_prev == o) ||
-                                          k - c_seen > 60000;
+                    const bool conflict = pf_last > pf_seen || (pf_stale && ord_prev == o) ||
+                                          k - pf_seen > 60000;
                     // position inside the node: u * root minus everything before it
-                    double pre = c_pre;
-                    if (c_stale && ord_prev < o) pre -= p_prev; // the update not yet in the tables
+                    double pre = pf_phi + pf_plo;
+                    if (pf_stale && ord_prev < o) pre -= p_prev; // the update not yet in the tables
                     const double pos = rootA * uk - pre;
-                    const double mass = (c_stale && ord_prev == o) ? c_mass - p_prev : c_mass;
+                    const double mass = (pf_stale && ord_prev == o) ? pf_mass - p_prev : pf_mass;
                     // one vote against the window in registers: leaf c, accepted only with pos
                     // farther than EPS inside [lo_c, hi_c)
-                    const int c = __popc(__ballot_sync(0xffffffffu, pos >= c_wlo)) - 1;
+                    const int c = __popc(__ballot_sync(0xffffffffu, pos >= pf_wlo)) - 1;
                     const int cs = c < 0 ? 0 : c;
-                    const double lo = __shfl_sync(0xffffffffu, c_wlo, cs);
-                    const double nx = __shfl_sync(0xffffffffu, c_wlo, (cs + 1) & 31);
-                    const double pr = __shfl_sync(0xffffffffu, c_wpr, cs);
-                    const double hi = cs == 31 ? c_wend : nx;
+                    const double lo = __shfl_sync(0xffffffffu, pf_wlo, cs);
+                    const double nx = __shfl_sync(0xffffffffu, pf_wlo, (cs + 1) & 31);
+                    const double pr = __shfl_sync(0xffffffffu, pf_wpr, cs);
+                    const double hi = cs == 31 ? pf_wend : nx;
                     if (!conflict && c >= 0 && pos > eps && pos < mass - eps && pos - lo > eps &&
                         hi - pos > eps) {
                         fast = true;
                         ord = o;
-                        rel = NLEAF + c_wfirst + c;
+                        rel = NLEAF + pf_wfirst + c;
                         prio = pr;
                         nfast++;
                     }
@@ -1600,11 +1608,22 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
                 // below (RING > NBUF draws back) is free.  The check cost this warp ~60 cycles
                 // per draw: its acquire load queued behind the previous draw's stores.
                 const long long tm3 = V6_CLK();
-                // ---- loads first: this draw's table entries
+                // ---- loads first: this draw's table entries (issued first: the stores wait
+                // for them), then the next draw's table entries and window, then the ready word
+                // of the draw after it.  A scout that releases a draw after its ready word was
+                // read costs the reload at the top of that draw.
                 const int base = ord & ~63, within = ord & 63, bk = ord >> 6;
                 const double t_m = mtab[ord];
                 const double t_l0 = plo[base + lane], t_l1 = plo[base + lane + 32];
                 const double t_h0 = phi[lane], t_h1 = phi[lane + 32];
+                asm volatile("" ::: "memory"); // keeps the loads above ahead of the prefetch
+                const long long tmp = V6_CLK();
+                if (k + 1 < a.n) {
+                    prefetch_from(k + 1, nx_wv);
+                    pf_stale = true;
+                }
+                if (k + 2 < a.n) nx_wv = ready_word(k + 2);
+                c_pref += V6_CLK() - tmp;
                 // ---- then the stores: ascent queue, publisher ring, approximate tables
                 const long long tm4 = V6_CLK();
                 if (lane == 0) {
@@ -1646,6 +1665,9 @@ __device__ __forceinline__ void exact_deep_v6(const SampleArgs &a, double *smem_
             a.dbg_cycles[2] = c_queue;
             a.dbg_cycles[3] = c_loads;
             a.dbg_cycles[4] = c_stores;
+            a.dbg_cycles[5] = c_late;
+            a.dbg_cycles[6] = n_late;
+            a.dbg_cycles[7] = c_pref;
         }
         if (lane == 0) a.st->pad = (nfast & 0xffff) | (nslow << 16); // fast draws, slow draws
     } else if (v6_ascent_id(warp) >= 0) {

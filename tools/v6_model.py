@@ -94,12 +94,23 @@ def leaf_window(E, node, D, x, shift=0):
     return lo, base + incl[-1], f
 
 
-def run(leaves, us, T, eps_rel=None, older=2, mispredict=0.0, rng=None):
+def run(leaves, us, T, eps_rel=None, older=2, mispredict=0.0, rng=None, prefetch=False,
+        stats=None):
     """Prefix-table formulation of the kernel: M / P_lo / P_hi over the level-(T-1)
     nodes in descent order (older half first), the scout's leaf window under the
     predicted node; a draw is accepted only when pos is farther than EPS from both ends
     of the node's interval and of the leaf's interval.  eps_rel=None is the kernel's
-    EPS = (n + 64) 2^-46 root for a launch of n = len(us) draws."""
+    EPS = (n + 64) 2^-46 root for a launch of n = len(us) draws.
+
+    prefetch=True models the main warp's pipeline: a draw's table entries are read before
+    the previous draw's update is stored, and that one update is applied in registers
+    (the prefix loses its priority when the previous node comes first in descent order; a
+    draw at the previous draw's node is a conflict and takes the exact path).  The scout's
+    window is then laid down from a staged copy of the exact tree that still lacks the
+    previous draw, as a copy taken before that draw was applied does in the kernel: a
+    decision at that node on that window can pick another leaf than the exact chain, which
+    is what the conflict rule prevents.  stats, a dict, receives counts of the draws decided
+    on corrected entries."""
     n = len(leaves)
     L = n.bit_length() - 1          # leaves at level L
     E = build(leaves)
@@ -120,6 +131,13 @@ def run(leaves, us, T, eps_rel=None, older=2, mispredict=0.0, rng=None):
             P_lo[b * blk + i] = r
             r += M[b * blk + i]
         run_hi += r
+    def apply_update(od, prio):
+        """approximate update: everything after the drawn node"""
+        M[od] -= prio
+        bb = od // blk
+        P_lo[od + 1:(bb + 1) * blk] -= prio
+        P_hi[bb + 1:] -= prio
+
     rootA = E[1]
     if eps_rel is None:
         eps_rel = (len(us) + 64) * 2.0 ** -46
@@ -128,6 +146,10 @@ def run(leaves, us, T, eps_rel=None, older=2, mispredict=0.0, rng=None):
     assert D >= 5, "the window holds 32 leaves: at least 5 levels below the table level"
     fallbacks = 0
     out = []
+    pending = None                  # (node, priority) of the draw whose update is not stored
+    E_staged = E.copy()             # the exact tree without the pending draw (prefetch=True)
+    if stats is not None:
+        stats.update(before=0, after=0, same=0, accepted_before=0, accepted_after=0)
     for u in us:
         want = exact_draw(Ex, n, u, older)
         # ---- scout: predicted node and leaf from the tables (optionally perturbed)
@@ -142,30 +164,49 @@ def run(leaves, us, T, eps_rel=None, older=2, mispredict=0.0, rng=None):
         if rng is not None and rng.rand() < mispredict:
             shift = int(rng.randint(-40, 41))
         node = ntop + (o ^ flip)
-        lo, end, f = leaf_window(E, node, D, x, shift)
+        lo, end, f = leaf_window(E_staged if prefetch else E, node, D, x, shift)
         # ---- main: one vote against the window
-        pos12 = fma_sub(rootA, u, P_hi[o // blk] + P_lo[o])
+        pre = P_hi[o // blk] + P_lo[o]
+        mass = M[o]
+        conflict = False
+        side = None
+        if pending is not None:     # the entries were read before the pending update
+            op, pp = pending
+            if op < o:
+                pre -= pp
+            conflict = op == o
+            side = "before" if op < o else "same" if op == o else "after"
+            apply_update(op, pp)
+            pending = None
+        pos12 = fma_sub(rootA, u, pre)
         leaf = None
-        if eps < pos12 < M[o] - eps:
+        if not conflict and eps < pos12 < mass - eps:
             c = int(np.count_nonzero(pos12 >= lo)) - 1
             hi = end if c == WIN - 1 else lo[min(c + 1, WIN - 1)]
             if c >= 0 and pos12 - lo[c] > eps and hi - pos12 > eps:
                 leaf = (node << D) + f + c
+        if stats is not None and side is not None:
+            stats[side] += 1
+            if leaf is not None and side != "same":
+                stats["accepted_" + side] += 1
         if leaf is None:
             fallbacks += 1
             leaf = exact_draw(E, n, u, older)
         assert leaf == want, ("decision differs from the exact chain", leaf, want, u)
         prio = E[leaf]
         out.append(leaf)
+        if prefetch:
+            E_staged = E.copy()
         zero_and_reduce(E, leaf)      # exact ascent (ascent warp)
         zero_and_reduce(Ex, leaf)
-        # approximate update: everything after the drawn node
         od = ((leaf >> D) - ntop) ^ flip
-        M[od] -= prio
-        bb = od // blk
-        P_lo[od + 1:(bb + 1) * blk] -= prio
-        P_hi[bb + 1:] -= prio
+        if prefetch:
+            pending = (od, prio)
+        else:
+            apply_update(od, prio)
         rootA = rootA - prio
+    if pending is not None:
+        apply_update(*pending)
     assert np.array_equal(E, Ex)
     return out, fallbacks
 

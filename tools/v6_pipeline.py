@@ -7,7 +7,10 @@ B2RL_V6_CYCLES=1 (1 M-leaf tree, B = 512, one k_replay_step launch per pass) and
 with the card name and power limit:
 
   main    own work: decide + table loads + stores; waits: for its scout (the next draw's
-          staging), and the segment that held the ascent-queue check (now the root update only)
+          staging), and the segment that held the ascent-queue check (now the root update only);
+          the scout wait split into draws whose staging was not yet released when it was
+          prefetched (spin and reload, and how many such draws) and the issue of the next
+          draw's prefetch, which waits for its ready word
   ascent  work and wait per draw, summed over the V6_NASC ascent warps; the warps apply
           draws side by side, so the draw period they set is work / V6_NASC
   scouts  fast / slow draws of the last pass
@@ -64,6 +67,17 @@ def main():
     from pfrl_b200 import _lib
 
     _lib.LIB_PATH = lib
+    # bench.py reports a fixed subset of b2rl_step_times; keep the whole array of the last call
+    L = _lib.load()
+    step_times = L.b2rl_step_times
+    raw = []
+
+    def keep_step_times(h, ph, stream):
+        st = step_times(h, ph, stream)
+        raw[:] = list(ph)
+        return st
+
+    L.b2rl_step_times = keep_step_times
     import bench
 
     sys.argv = ["bench.py", "--no-rainbow", "--no-secondary", "--no-cpu-baseline",
@@ -80,11 +94,14 @@ def main():
     s = line["sampler"]
     na = nasc()
     main_work = c["main_decide"] + c["main_loads"] + c["main_stores"]
+    B = line["config"]["batch_per_rank"]
+    late, n_late, pref = raw[9] / B, raw[10], raw[11] / B  # dbg_cycles [5], [6], [7]
     res = {
         "card": card(),
         "ascent_warps": na,
         "main": {"own_work": main_work, "decide": c["main_decide"], "loads": c["main_loads"],
                  "stores": c["main_stores"], "wait_scout": c["main_wait_scout"],
+                 "late_scout": late, "late_draws": n_late, "prefetch_next": pref,
                  "wait_queue": c["main_wait_queue"]},
         "ascent": {"work_per_draw": c["ascent_work"], "wait_per_draw": c["ascent_wait"],
                    "work_per_draw_period": c["ascent_work"] / na},
@@ -96,11 +113,13 @@ def main():
     with open(os.path.join(args.out, "v6_pipeline.json"), "w") as f:
         json.dump(res, f, indent=1)
     print("card: %s" % res["card"])
-    print("cycles per draw (last launch, B = %d):" % line["config"]["batch_per_rank"])
+    print("cycles per draw (last launch, B = %d):" % B)
     print("  main    own work %6.0f  (decide %.0f, table loads %.0f, stores %.0f)"
           % (main_work, c["main_decide"], c["main_loads"], c["main_stores"]))
     print("          waits    for its scout %.0f, queue segment %.0f"
           % (c["main_wait_scout"], c["main_wait_queue"]))
+    print("          scout not released at the prefetch: %.0f (%d of %d draws); issuing the next"
+          " draw's prefetch: %.0f" % (late, n_late, B, pref))
     print("  ascent  work %6.0f per draw over %d warps = %.0f per draw period; wait %.0f"
           % (c["ascent_work"], na, c["ascent_work"] / na, c["ascent_wait"]))
     print("  draw period (main work + waits) %.0f; sampling phase %.1f us"
