@@ -459,6 +459,51 @@ int b2rl_adv_td_loss_fwd(int mode, const float *q, const int64_t *action,
                          float *delta_out, float *scratch, float *loss_out,
                          void *stream);
 
+/* NAF head (FCQuadraticStateQFunction): L with L[i][i] = exp(diag_pre[i]) and
+ * the n(n-1)/2 entries of non_diag below the diagonal in np.tril_indices(n, -1)
+ * order; mat = L L^T [B,n,n].  non_diag may be NULL when n = 1.  The backward
+ * takes grad_mat (any, not assumed symmetric) and writes the gradients of
+ * diag_pre and non_diag.  Any n. */
+int b2rl_naf_head_fwd(const float *diag_pre, const float *non_diag, int32_t B,
+                      int32_t n, float *mat, void *stream);
+int b2rl_naf_head_bwd(const float *diag_pre, const float *non_diag,
+                      const float *grad_mat, int32_t B, int32_t n,
+                      float *grad_diag_pre, float *grad_non_diag, void *stream);
+
+/* TD loss of the DQN family with a QuadraticActionValue (NAF):
+ * Q(u) = v - 1/2 (u - mu)^T P (u - mu), max = v when neither bound is given,
+ * else Q(clamp(mu)).  y = Q(s, a) from (mu, mat, v) of the online net at s;
+ * (tmu, tmat, tv) and (tnmu, tnmat, tnv) the target net at s and s'; nmu the
+ * online net's mu at s'; lo / hi the target net's bounds and nlo / nhi the
+ * online net's ([n] each, any may be NULL).  T = r + discount*(1-terminal)*nextV.
+ *   NAF_DQN         nextV = max'(s')              t = T
+ *   NAF_DOUBLE_DQN  nextV = Q'(s', clamp(nmu))    t = T
+ *   ADV_AL          nextV = max'(s')              t = T + alpha*A'(s, a)
+ *   ADV_PAL         nextV = max'(s')              t = T + alpha*max(A'(s,a), A'(s',a))
+ *   ADV_DOUBLE_PAL  nextV = Q'(s', clamp(nmu))    t as PAL
+ *   ADV_DPP_GREEDY  nextV = max'(s')              t = Q'(s, a) + T - max'(s)
+ * with A'(x, a) = Q'(x, a) - max'(x).  tmu/tmat/tv are needed except for the
+ * DQN modes, nmu for the double modes.  Outputs as b2rl_td_loss_fwd.  The
+ * backward writes d loss / d (mu, mat, v) of the online net at s. */
+#define B2RL_NAF_DQN 6
+#define B2RL_NAF_DOUBLE_DQN 7
+int b2rl_naf_td_loss_fwd(int mode, const float *mu, const float *mat,
+                         const float *v, const float *action, const float *tmu,
+                         const float *tmat, const float *tv, const float *tnmu,
+                         const float *tnmat, const float *tnv, const float *nmu,
+                         const float *lo, const float *hi, const float *nlo,
+                         const float *nhi, const float *reward,
+                         const float *discount, const float *terminal,
+                         const float *weights, int32_t B, int32_t n,
+                         double alpha, int clip_delta, int mean, float *y_out,
+                         float *t_out, float *delta_out, float *scratch,
+                         float *loss_out, void *stream);
+int b2rl_naf_td_loss_bwd(const float *mu, const float *mat, const float *action,
+                         const float *y, const float *t, const float *weights,
+                         const float *grad_loss, int32_t B, int32_t n,
+                         int clip_delta, int mean, float *grad_mu,
+                         float *grad_mat, float *grad_v, void *stream);
+
 /* Quantile Huber loss of IQN: |tau - 1[t<y]| * Huber(y, t) over [B, N, N'],
  * mean over N', sum over N (compute_eltwise_huber_quantile_loss and the value
  * losses of pfrl/agents/iqn.py:176-250); delta_out = mean over (N, N'). */

@@ -21,6 +21,7 @@ from pfrl_b200 import envs  # NOQA
 from pfrl_b200 import experiments  # NOQA
 from pfrl_b200 import explorer  # NOQA
 from pfrl_b200 import explorers  # NOQA
+from pfrl_b200 import functions  # NOQA
 from pfrl_b200 import initializers  # NOQA
 from pfrl_b200 import nn  # NOQA
 from pfrl_b200 import optimizers  # NOQA

@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 LIB_PATH = os.path.join(CSRC, "libb2rl.so")
-SOURCES = ["replay.cu", "sampler.cu", "step.cu", "gather.cu", "episodic.cu", "rollout.cu", "losses.cu", "ppo.cu", "trpo.cu", "acer.cu", "reinforce.cu", "sac.cu", "conv.cu", "gemm.cu"]
+SOURCES = ["replay.cu", "sampler.cu", "step.cu", "gather.cu", "episodic.cu", "rollout.cu", "losses.cu", "ppo.cu", "trpo.cu", "acer.cu", "reinforce.cu", "naf.cu", "sac.cu", "conv.cu", "gemm.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
@@ -38,6 +38,7 @@ def build(force=False, verbose=False):
     """Compile libb2rl.so in-tree with nvcc for sm_90a (no GPU needed)."""
     srcs = _sources()
     deps = srcs + [os.path.join(CSRC, "b2rl_internal.cuh"), os.path.join(CSRC, "tree_dev.cuh"),
+                   os.path.join(CSRC, "td_common.cuh"),
                    os.path.join(INCLUDE, "b2rl.h")]
     if (
         not force
@@ -223,6 +224,11 @@ SIGNATURES = {
     "b2rl_td_loss_bwd": (_int, [_vp] * 5 + [_i32, _i32, _int, _int, _vp, _vp]),
     "b2rl_adv_td_loss_fwd": (_int, [_int] + [_vp] * 9 + [_i32, _i32, _dbl, _dbl, _int, _int]
                              + [_vp] * 6),
+    "b2rl_naf_head_fwd": (_int, [_vp, _vp, _i32, _i32, _vp, _vp]),
+    "b2rl_naf_head_bwd": (_int, [_vp] * 3 + [_i32, _i32] + [_vp] * 3),
+    "b2rl_naf_td_loss_fwd": (_int, [_int] + [_vp] * 19 + [_i32, _i32, _dbl, _int, _int]
+                             + [_vp] * 6),
+    "b2rl_naf_td_loss_bwd": (_int, [_vp] * 7 + [_i32, _i32, _int, _int] + [_vp] * 4),
     "b2rl_quantile_huber_fwd": (_int, [_vp] * 4 + [_i32, _i32, _i32, _int] + [_vp] * 4),
     "b2rl_quantile_huber_bwd": (_int, [_vp] * 5 + [_i32, _i32, _i32, _int, _vp, _vp]),
     "b2rl_gae": (_int, [_vp] * 6 + [_i32, _i32, _dbl, _dbl] + [_vp] * 5),

@@ -178,6 +178,83 @@ class QuantileDiscreteActionValue(DiscreteActionValue):
         return QuantileDiscreteActionValue(self.quantiles[i], self.q_values_formatter)
 
 
+def _as_bound(b, device):
+    """A bound as an fp32 tensor on ``device``: a scalar becomes [b]; a tensor already there
+    in fp32 is used as it is, so no copy is made per forward (and the Q-function can be
+    captured in a CUDA graph)."""
+    if b is None:
+        return None
+    if isinstance(b, torch.Tensor) and b.device == device and b.dtype == torch.float32:
+        return b
+    if isinstance(b, (int, float)):
+        b = [b]
+    return torch.as_tensor(b).to(device).float()
+
+
+class QuadraticActionValue(ActionValue):
+    """Q(s, u) = V(s) - 1/2 (u - mu(s))^T P(s) (u - mu(s)) for continuous actions (NAF,
+    arXiv:1603.00748; pfrl/action_value.py QuadraticActionValue).
+
+    ``mu`` [batch, n] maximises the advantage, ``mat`` [batch, n, n] is P (positive definite
+    when it comes from a NAF head), ``v`` [batch, 1] or [batch].  ``min_action`` and
+    ``max_action`` (scalar, sequence, ndarray or tensor; not batched) clamp the greedy
+    action; ``max`` is ``v`` without bounds and Q at the greedy action with them."""
+
+    def __init__(self, mu, mat, v, min_action=None, max_action=None):
+        self.mu = mu
+        self.mat = mat
+        self.v = v
+        self.device = mu.device
+        self.min_action = _as_bound(min_action, self.device)
+        self.max_action = _as_bound(max_action, self.device)
+        self.batch_size = self.mu.shape[0]
+        self._greedy = self._max = None
+
+    @property
+    def greedy_actions(self):
+        if self._greedy is None:
+            a = self.mu
+            if self.min_action is not None:
+                a = torch.max(self.min_action.unsqueeze(0).expand_as(a), a)
+            if self.max_action is not None:
+                a = torch.min(self.max_action.unsqueeze(0).expand_as(a), a)
+            self._greedy = a
+        return self._greedy
+
+    @property
+    def max(self):
+        if self._max is None:
+            if self.min_action is None and self.max_action is None:
+                self._max = self.v.reshape(self.batch_size)
+            else:
+                self._max = self.evaluate_actions(self.greedy_actions)
+        return self._max
+
+    def evaluate_actions(self, actions):
+        u_minus_mu = actions - self.mu
+        a = -0.5 * torch.matmul(torch.matmul(u_minus_mu[:, None, :], self.mat),
+                                u_minus_mu[:, :, None])[:, 0, 0]
+        return a + self.v.reshape(self.batch_size)
+
+    def compute_advantage(self, actions):
+        return self.evaluate_actions(actions) - self.max
+
+    def compute_double_advantage(self, actions, argmax_actions):
+        return self.evaluate_actions(actions) - self.evaluate_actions(argmax_actions)
+
+    def __repr__(self):
+        return "QuadraticActionValue greedy_actions:{} v:{}".format(
+            self.greedy_actions.detach().cpu().numpy(), self.v.detach().cpu().numpy())
+
+    @property
+    def params(self):
+        return (self.mu, self.mat, self.v)
+
+    def __getitem__(self, i):
+        return QuadraticActionValue(self.mu[i], self.mat[i], self.v[i],
+                                    min_action=self.min_action, max_action=self.max_action)
+
+
 class SingleActionValue(ActionValue):
     """Action value known only through callables: ``evaluator(actions)`` scores
     given actions, ``maximizer()`` returns the greedy ones (continuous-action

@@ -6,6 +6,8 @@ class DoubleDQN(dqn.DQN):
     """Double DQN (arXiv:1509.06461): the online network picks the next
     action, the target network evaluates it (pfrl/agents/double_dqn.py:12-40)."""
 
+    _fused_mode = "double_dqn"
+
     def _next_q(self, exp_batch):
         # recurrent: both forwards run over the packed next states from the
         # batch's next_recurrent_state (double_dqn.py:15-32)

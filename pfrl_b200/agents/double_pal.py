@@ -13,9 +13,10 @@ class DoublePAL(pal.PAL):
 
     _fused_mode = "double_pal"
 
-    def _compute_y_and_t(self, exp_batch):
+    def _compute_y_and_t(self, exp_batch, qout=None):
         # forwards in the reference's order: online(s), online(s'), target(s), target(s')
-        qout = self.model(exp_batch["state"])
+        if qout is None:  # the fused path hands in its own forward at s
+            qout = self.model(exp_batch["state"])
         y = qout.evaluate_actions(exp_batch["action"])
         with torch.no_grad():
             next_qout = self.model(exp_batch["next_state"])

@@ -30,12 +30,13 @@ class AbstractDPP(DQN, metaclass=ABCMeta):
         return exp_batch["reward"] + exp_batch["discount"] * (
             1.0 - exp_batch["is_state_terminal"]) * next_l
 
-    def _compute_y_and_t(self, exp_batch):
+    def _compute_y_and_t(self, exp_batch, qout=None):
         batch_size = exp_batch["reward"].shape[0]
         action = exp_batch["action"]
         # forwards in the reference's order: online(s), target(s), then target(s') in
         # _compute_target_values
-        qout = self.model(exp_batch["state"])
+        if qout is None:  # the fused path hands in its own forward at s
+            qout = self.model(exp_batch["state"])
         y = qout.evaluate_actions(action).reshape(batch_size, 1)
         with torch.no_grad():
             target_qout = self.target_model(exp_batch["state"])

@@ -30,6 +30,8 @@ import torch
 import torch.nn.functional as F
 
 from pfrl_b200 import _lib, agent
+from pfrl_b200.action_value import QuadraticActionValue
+from pfrl_b200.agents import _advantage
 from pfrl_b200.agents._graph import CapturedStep
 from pfrl_b200.ops import losses as fused
 from pfrl_b200.replay_buffer import (
@@ -347,12 +349,17 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
 
     use_fused_loss = True
 
+    # the target the NAF kernel computes for this class (agents._advantage.fused_mode)
+    _fused_mode = "dqn"
+
     def _compute_loss(self, exp_batch, want_errors=False):
         """Returns (loss, per-sample |y - t| or None); dqn.py:432-470."""
         if self.use_fused_loss and exp_batch["reward"].is_cuda:
             # one fused kernel: gather Q(s)[a], TD target, |y - t|, Huber / MSE,
             # importance weights and the deterministic batch reduction
             qout = self._forward(self.model, exp_batch, "state")
+            if isinstance(qout, QuadraticActionValue):
+                return self._compute_naf_loss(exp_batch, qout, want_errors)
             with torch.no_grad():
                 next_q = self._next_q(exp_batch)
             loss, delta, y, _ = fused.td_loss(
@@ -364,9 +371,26 @@ class DQN(agent.AttributeSavingMixin, agent.BatchAgent):
             return loss, delta
         return self._compute_loss_torch(exp_batch, want_errors)
 
+    def _compute_naf_loss(self, exp_batch, qout, want_errors):
+        """Loss of a continuous-action (NAF) Q-function whose output at s is ``qout``: the NAF
+        kernel where it computes this class's target from fp32 values, else the reference's
+        target in torch (after the same forward at s)."""
+        mode = _advantage.fused_mode(self)
+        if (mode in ("dqn", "double_dqn") and not self.recurrent
+                and _advantage.naf_kernel_dtypes(qout)):
+            return _advantage.naf_loss(self, exp_batch, qout, mode)
+        batch_size = exp_batch["reward"].shape[0]
+        y = torch.reshape(qout.evaluate_actions(exp_batch["action"]), (batch_size, 1))
+        with torch.no_grad():
+            t = torch.reshape(self._compute_target_values(exp_batch), (batch_size, 1))
+        return self._value_loss(y, t, exp_batch, want_errors)
+
     def _compute_loss_torch(self, exp_batch, want_errors=False):
         """The reference's formulation: _compute_y_and_t, then the value loss."""
         y, t = self._compute_y_and_t(exp_batch)
+        return self._value_loss(y, t, exp_batch, want_errors)
+
+    def _value_loss(self, y, t, exp_batch, want_errors):
         self._last_q = y.detach()
         delta = None
         if want_errors:

@@ -30,9 +30,10 @@ class PAL(dqn.DQN):
                               target_next_qout.compute_advantage(action))
         return bellman + self.alpha * advantage
 
-    def _compute_y_and_t(self, exp_batch):
+    def _compute_y_and_t(self, exp_batch, qout=None):
         # forwards in the reference's order: online(s), target(s), target(s')
-        qout = self.model(exp_batch["state"])
+        if qout is None:  # the fused path hands in its own forward at s
+            qout = self.model(exp_batch["state"])
         y = qout.evaluate_actions(exp_batch["action"])
         with torch.no_grad():
             target_qout = self.target_model(exp_batch["state"])

@@ -16,43 +16,9 @@
 #include <math.h>
 
 #include "b2rl_internal.cuh"
+#include "td_common.cuh"
 
 namespace {
-
-__device__ unsigned int g_done_counter[B2RL_N_TICKETS]; // zero-initialised, self-resetting
-
-__device__ __forceinline__ float warp_sum(float v)
-{
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
-// Deterministic final reduction: the last CTA to arrive sums term[i] for
-// i < n in a fixed order and writes *out = sum / divisor.
-__device__ void finish_sum(const float *term, int n, float divisor, float *out, float *sh,
-                           unsigned ticket)
-{
-    __shared__ bool last;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        const unsigned int prev = atomicInc(&g_done_counter[ticket], gridDim.x - 1);
-        last = (prev == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
-    float s = 0.f;
-    for (int i = threadIdx.x; i < n; i += blockDim.x) s += __ldcg(term + i);
-    s = warp_sum(s);
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        s = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.f;
-        s = warp_sum(s);
-        if (threadIdx.x == 0) *out = __fdiv_rn(s, divisor);
-    }
-}
 
 // ---------------------------------------------------------------------------
 // C51: one warp per sample.
@@ -149,31 +115,6 @@ struct TdArgs {
     float *y_out, *t_out, *delta_out, *term, *loss_out;
     unsigned ticket;
 };
-
-// r + discount * (1 - terminal) * next_v, dqn.py:405
-__device__ __forceinline__ float bellman_target(float r, float discount, float terminal,
-                                                float next_v)
-{
-    return __fadd_rn(r, __fmul_rn(__fmul_rn(discount, __fsub_rn(1.0f, terminal)), next_v));
-}
-
-// Writes y, t, |y - t| and the (weighted) Huber / 0.5 MSE term of sample i (dqn.py:44-104).
-__device__ __forceinline__ void td_outputs(float y, float t, int i, int clip_delta,
-                                           const float *weights, float *y_out, float *t_out,
-                                           float *delta_out, float *term)
-{
-    const float d = __fsub_rn(y, t);
-    const float ad = fabsf(d);
-    float l;
-    if (clip_delta)
-        l = ad < 1.0f ? __fmul_rn(__fmul_rn(0.5f, d), d) : __fsub_rn(ad, 0.5f);
-    else
-        l = __fmul_rn(__fmul_rn(d, d), 0.5f);
-    y_out[i] = y;
-    t_out[i] = t;
-    delta_out[i] = ad;
-    term[i] = weights ? __fmul_rn(l, weights[i]) : l;
-}
 
 __global__ void __launch_bounds__(256) k_td_fwd(TdArgs a)
 {
@@ -314,14 +255,8 @@ __global__ void k_td_bwd(TdBwdArgs a)
     if (idx >= a.B * a.nA) return;
     const int i = idx / a.nA, j = idx - i * a.nA;
     float gq = 0.f;
-    if (j == (int)a.action[i]) {
-        float g = a.grad_loss[0];
-        if (a.mean) g = g / (float)a.B;
-        if (a.weights) g *= a.weights[i];
-        float d = a.y[i] - a.t[i];
-        if (a.clip_delta) d = fminf(fmaxf(d, -1.0f), 1.0f); // Huber'(d), delta = 1
-        gq = g * d;
-    }
+    if (j == (int)a.action[i])
+        gq = td_grad(a.y, a.t, a.weights, a.grad_loss, i, a.B, a.clip_delta, a.mean);
     a.grad_q[idx] = gq;
 }
 

@@ -3,6 +3,7 @@ from pfrl_b200.q_functions.state_q_functions import (  # NOQA
     DiscreteActionValueHead,
     DistributionalFCStateQFunctionWithDiscreteAction,
     DistributionalSingleModelStateQFunctionWithDiscreteAction,
+    FCQuadraticStateQFunction,
     FCStateQFunctionWithDiscreteAction,
     SingleModelStateQFunctionWithDiscreteAction,
 )

@@ -5,7 +5,11 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from pfrl_b200.action_value import DiscreteActionValue, DistributionalDiscreteActionValue
+from pfrl_b200.action_value import (
+    DiscreteActionValue, DistributionalDiscreteActionValue, QuadraticActionValue,
+)
+from pfrl_b200.functions.lower_triangular_matrix import lower_triangular_matrix
+from pfrl_b200.initializers import init_chainer_default
 from pfrl_b200.nn.mlp import MLP
 from pfrl_b200.q_function import StateQFunction
 
@@ -71,6 +75,77 @@ class DistributionalFCStateQFunctionWithDiscreteAction(
                 last_wscale=last_wscale),
             _Head())
         super().__init__(model=model, z_values=z_values)
+
+
+class FCQuadraticStateQFunction(nn.Module, StateQFunction):
+    """NAF Q-function for continuous actions (arXiv:1603.00748;
+    pfrl/q_functions/state_q_functions.py FCQuadraticStateQFunction): ReLU hidden layers, then
+    linear heads for V, mu (scaled into the action box by tanh when ``scale_mu``) and the
+    diagonal and lower part of L, with P = L L^T.  Same parameters and ``state_dict`` keys as
+    the reference.
+
+    The tanh scale and mean and the action bounds are non-persistent buffers: they follow the
+    module to its device once instead of being copied from the host on every forward.  On CUDA
+    with fp32 parameters, P is built by one kernel (ops.naf.head); elsewhere by the
+    reference's torch formulation."""
+
+    def __init__(self, n_input_channels, n_dim_action, n_hidden_channels, n_hidden_layers,
+                 action_space, scale_mu=True):
+        self.n_input_channels = n_input_channels
+        self.n_hidden_layers = n_hidden_layers
+        self.n_hidden_channels = n_hidden_channels
+        self.n_dim_action = n_dim_action
+        assert action_space is not None
+        self.scale_mu = scale_mu
+        self.action_space = action_space
+        super().__init__()
+        hidden_layers = nn.ModuleList()
+        assert n_hidden_layers >= 1
+        hidden_layers.append(init_chainer_default(nn.Linear(n_input_channels, n_hidden_channels)))
+        for _ in range(n_hidden_layers - 1):
+            hidden_layers.append(
+                init_chainer_default(nn.Linear(n_hidden_channels, n_hidden_channels)))
+        self.hidden_layers = hidden_layers
+
+        self.v = init_chainer_default(nn.Linear(n_hidden_channels, 1))
+        self.mu = init_chainer_default(nn.Linear(n_hidden_channels, n_dim_action))
+        self.mat_diag = init_chainer_default(nn.Linear(n_hidden_channels, n_dim_action))
+        non_diag_size = n_dim_action * (n_dim_action - 1) // 2
+        if non_diag_size > 0:
+            self.mat_non_diag = init_chainer_default(nn.Linear(n_hidden_channels, non_diag_size))
+
+        high, low = action_space.high, action_space.low
+        # scale_by_tanh's numpy arithmetic, as the reference does it per forward
+        self.register_buffer("mu_scale", torch.from_numpy(np.asarray((high - low) / 2))[None],
+                             persistent=False)
+        self.register_buffer("mu_mean", torch.from_numpy(np.asarray((high + low) / 2))[None],
+                             persistent=False)
+        self.register_buffer("min_action", torch.as_tensor(low).float(), persistent=False)
+        self.register_buffer("max_action", torch.as_tensor(high).float(), persistent=False)
+
+    def forward(self, state):
+        h = state
+        for layer in self.hidden_layers:
+            h = F.relu(layer(h))
+        v = self.v(h)
+        mu = self.mu(h)
+        if self.scale_mu:
+            mu = torch.tanh(mu) * self.mu_scale + self.mu_mean
+        diag_pre = self.mat_diag(h)
+        non_diag = self.mat_non_diag(h) if hasattr(self, "mat_non_diag") else None
+        if diag_pre.is_cuda and diag_pre.dtype == torch.float32:
+            from pfrl_b200.ops import naf
+
+            mat = naf.head(diag_pre, non_diag)
+        else:
+            mat_diag = torch.exp(diag_pre)
+            if non_diag is not None:
+                tril = lower_triangular_matrix(mat_diag, non_diag)
+                mat = torch.matmul(tril, torch.transpose(tril, 1, 2))
+            else:
+                mat = torch.unsqueeze(mat_diag ** 2, dim=2)
+        return QuadraticActionValue(mu, mat, v, min_action=self.min_action,
+                                    max_action=self.max_action)
 
 
 class DiscreteActionValueHead(nn.Module):

@@ -40,7 +40,8 @@ wrappers.VectorFrameStack wrappers.atari_wrappers.FrameStack wrappers.atari_wrap
 collections.prioritized.PrioritizedBuffer collections.random_access_queue.RandomAccessQueue
 optimizers.RMSpropEpsInsideSqrt action_value.DiscreteActionValue
 action_value.DistributionalDiscreteActionValue action_value.QuantileDiscreteActionValue
-action_value.SingleActionValue
+action_value.SingleActionValue action_value.QuadraticActionValue
+q_functions.FCQuadraticStateQFunction functions.lower_triangular_matrix.lower_triangular_matrix
 """.split()
 
 METHOD_CLASSES = """
@@ -52,6 +53,7 @@ envs.MultiprocessVectorEnv envs.SerialVectorEnv wrappers.VectorFrameStack
 action_value.DiscreteActionValue action_value.DistributionalDiscreteActionValue
 action_value.QuantileDiscreteActionValue explorers.LinearDecayEpsilonGreedy explorers.AdditiveOU
 collections.random_access_queue.RandomAccessQueue experiments.evaluator.Evaluator
+action_value.QuadraticActionValue q_functions.FCQuadraticStateQFunction
 """.split()
 
 # methods of the reference that belong to features outside the rebuilt path
