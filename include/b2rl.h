@@ -641,6 +641,24 @@ int b2rl_reinforce_loss(int64_t N, int32_t D, const float *z, const float *loc,
                         void *stream);
 
 /* ------------------------------------------------------------------------
+ * A3C's loss gradient over the N recorded steps of one segment
+ * (pfrl/agents/a3c.py:177-204): returns R from the fp64 scan R = R * gamma + r
+ * backwards from *bootstrap (NULL = terminal, R = 0), rounded to fp32;
+ * adv = R - v; loss = pi_factor * sum_rows(-adv log pi(a) - beta H)
+ * + v_factor * sum_rows((v - R)^2) / 2.  fp32 storage, fp64 arithmetic, device
+ * pointers, one warp per row.  The policy is given as for b2rl_reinforce_loss
+ * (z, actions and g_z, or loc, scale, action_values, g_loc and g_scale).
+ * v fp32 [N], rewards fp64 [N].  Writes g_v [N]; returns [N] (fp32) unless
+ * NULL; row_pi_loss and row_v_loss [N] (both or neither) take each row's
+ * term of pi_loss and v_loss. */
+int b2rl_a3c_loss(int64_t N, int32_t D, const float *z, const float *loc,
+                  const float *scale, const int64_t *actions,
+                  const float *action_values, const float *v, const double *rewards,
+                  const float *bootstrap, double gamma, double beta, double pi_factor,
+                  double v_factor, float *g_z, float *g_loc, float *g_scale, float *g_v,
+                  float *returns, float *row_pi_loss, float *row_v_loss, void *stream);
+
+/* ------------------------------------------------------------------------
  * SAC / TD3 / DDPG update tail (fp32, device pointers).
  * ---------------------------------------------------------------------- */
 

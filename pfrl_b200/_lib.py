@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 LIB_PATH = os.path.join(CSRC, "libb2rl.so")
-SOURCES = ["replay.cu", "sampler.cu", "step.cu", "gather.cu", "episodic.cu", "rollout.cu", "losses.cu", "ppo.cu", "trpo.cu", "acer.cu", "reinforce.cu", "naf.cu", "sac.cu", "conv.cu", "gemm.cu"]
+SOURCES = ["replay.cu", "sampler.cu", "step.cu", "gather.cu", "episodic.cu", "rollout.cu", "losses.cu", "ppo.cu", "trpo.cu", "acer.cu", "reinforce.cu", "a3c.cu", "naf.cu", "sac.cu", "conv.cu", "gemm.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
@@ -38,7 +38,7 @@ def build(force=False, verbose=False):
     """Compile libb2rl.so in-tree with nvcc for sm_90a (no GPU needed)."""
     srcs = _sources()
     deps = srcs + [os.path.join(CSRC, "b2rl_internal.cuh"), os.path.join(CSRC, "tree_dev.cuh"),
-                   os.path.join(CSRC, "td_common.cuh"),
+                   os.path.join(CSRC, "td_common.cuh"), os.path.join(CSRC, "pg_common.cuh"),
                    os.path.join(INCLUDE, "b2rl.h")]
     if (
         not force
@@ -242,6 +242,7 @@ SIGNATURES = {
     "b2rl_acer_loss": (_int, [_i32, _i32] + [_vp] * 7 + [_dbl, _i32, _dbl, _i32] + [_dbl] * 4
                        + [_i32, _i32, _vp, _dbl] + [_vp] * 4),
     "b2rl_reinforce_loss": (_int, [_i64, _i32] + [_vp] * 6 + [_i32, _dbl] + [_vp] * 6),
+    "b2rl_a3c_loss": (_int, [_i64, _i32] + [_vp] * 8 + [_dbl] * 4 + [_vp] * 8),
     "b2rl_polyak": (_int, [ctypes.POINTER(TensorPair), _i32, _dbl, _vp]),
     "b2rl_sac_target": (_int, [_vp] * 7 + [ctypes.c_float, _i32, _vp, _vp]),
     "b2rl_conv_nature1_fwd": (_int, [_vp, _vp, _vp, _i32, _vp, _vp]),

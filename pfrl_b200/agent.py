@@ -114,6 +114,34 @@ class AsyncAgent(Agent, metaclass=ABCMeta):
         pass
 
 
+def assert_shared_memory(agent, models=("model", "shared_model")):
+    """The check of an ``AsyncAgent``'s ``assert_shared_memory`` (pfrl/agents/a3c.py:
+    110-123).  On the CPU, the reference's: ``agent.shared_model`` and the optimizer's
+    state are in shared memory and ``agent.model`` is not.  CUDA storages always report
+    ``is_shared()``, so on CUDA what sharing is for is checked instead: the modules named in
+    ``models`` share no storage, and ``agent.optimizer`` steps ``agent.shared_model``'s
+    parameters."""
+    if agent.device.type != "cuda":
+        for k, v in agent.shared_model.state_dict().items():
+            assert v.is_shared(), "{} is not in shared memory".format(k)
+        for k, v in agent.model.state_dict().items():
+            assert not v.is_shared(), "{} is in shared memory".format(k)
+        for param_state in agent.optimizer.state_dict()["state"].values():
+            for k, v in param_state.items():
+                if isinstance(v, torch.Tensor):
+                    assert v.is_shared(), "{} is not in shared memory".format(k)
+        return
+    ptrs = {}
+    for name in models:
+        for k, v in getattr(agent, name).state_dict().items():
+            if v.numel():
+                owner = ptrs.setdefault(v.untyped_storage().data_ptr(), name)
+                assert owner == name, "{}.{} shares storage with {}".format(name, k, owner)
+    stepped = {id(p) for group in agent.optimizer.param_groups for p in group["params"]}
+    assert stepped == {id(p) for p in agent.shared_model.parameters()}, \
+        "the optimizer must step shared_model's parameters"
+
+
 class BatchAgent(Agent, metaclass=ABCMeta):
     """Agent that steps a batch of environments; the single-env calls are
     the batch calls with a batch of one (pfrl/agent.py:157-200)."""

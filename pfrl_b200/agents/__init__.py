@@ -15,3 +15,4 @@ from pfrl_b200.agents import ddpg  # NOQA  (module path of the reference)
 from pfrl_b200.agents.trpo import TRPO  # NOQA
 from pfrl_b200.agents.acer import ACER  # NOQA
 from pfrl_b200.agents.reinforce import REINFORCE  # NOQA
+from pfrl_b200.agents.a3c import A3C  # NOQA

@@ -283,26 +283,7 @@ class ACER(agent.AttributeSavingMixin, agent.AsyncAgent):
                                    source_link=self.model, tau=1 - self.trust_region_alpha)
 
     def assert_shared_memory(self):
-        if self.device.type != "cuda":
-            for k, v in self.shared_model.state_dict().items():
-                assert v.is_shared(), "{} is not in shared memory".format(k)
-            for k, v in self.model.state_dict().items():
-                assert not v.is_shared(), "{} is in shared memory".format(k)
-            for param_state in self.optimizer.state_dict()["state"].values():
-                for k, v in param_state.items():
-                    if isinstance(v, torch.Tensor):
-                        assert v.is_shared(), "{} is not in shared memory".format(k)
-            return
-        # CUDA storages always report is_shared(): check what sharing is for instead
-        ptrs = {}
-        for name in ("model", "shared_model", "shared_average_model"):
-            for k, v in getattr(self, name).state_dict().items():
-                if v.numel():
-                    owner = ptrs.setdefault(v.untyped_storage().data_ptr(), name)
-                    assert owner == name, "{}.{} shares storage with {}".format(name, k, owner)
-        stepped = {id(p) for group in self.optimizer.param_groups for p in group["params"]}
-        assert stepped == {id(p) for p in self.shared_model.parameters()}, \
-            "the optimizer must step shared_model's parameters"
+        agent.assert_shared_memory(self, ("model", "shared_model", "shared_average_model"))
 
     @property
     def shared_attributes(self):

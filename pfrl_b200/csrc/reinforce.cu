@@ -11,29 +11,20 @@
 // The backward of the reference's loss hands log pi(a) and H of one row the fp32 gradients
 //   c_lp = fl32(fl32(1 / batchsize) * fl32(-R)),   c_H = -fl32(fl32(1 / batchsize) * fl32(beta))
 // (DivBackward, then MulBackward with the Python / numpy scalar rounded to fp32, then the
-// subtraction's sign), and these are formed here in fp32 the same way.  Below them:
-//   Categorical, z = Categorical._param (normalised logits), p = softmax(z):
-//     d log pi(a) / dz = e_a (log_prob is a gather of z)
-//     H = -sum_j c_j p_j with c_j = max(z_j, finfo(fp32).min) (torch's clamp), so
-//     dH / dz_j = -p_j (m_j + c_j + H), m_j = [z_j >= finfo.min] (the clamp passes the gradient)
-//   Independent(Normal(loc, scale), 1), d = a - loc:
-//     d log pi / d loc = d / scale^2,  d log pi / d scale = d^2 / scale^3 - 1 / scale
-//     dH / d scale = 1 / scale,        dH / d loc = 0
-// Everything past the two coefficients is fp64, stored in fp32.
+// subtraction's sign), and these are formed here in fp32 the same way.  Below them, the
+// row's d log pi(a) and dH (pg_common.cuh, shared with a3c.cu) are fp64, stored in fp32.
 //
 // One warp per row, lanes striding the K categories or A action dimensions, rows striding the
 // grid: any N, K and A.  No shared memory, no scratch, no atomics: the output is deterministic.
-#include <float.h>
-#include <math.h>
 #include <stdint.h>
 
 #include "b2rl_internal.cuh"
+#include "pg_common.cuh"
 
 namespace {
 
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
-constexpr double kHalfLog2Pi = 0.91893853320467274178; // log(sqrt(2 pi))
 
 struct ReinforceArgs {
     int64_t N;
@@ -49,77 +40,24 @@ struct ReinforceArgs {
     float *row_loss, *row_ent;  // [N] each, optional
 };
 
-__device__ __forceinline__ double warp_sum(double v)
-{
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
-__device__ __forceinline__ double warp_max(double v)
-{
-    for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-
 __device__ void categorical_row(const ReinforceArgs &a, int64_t i, int lane, double c_lp,
                                 double c_h)
 {
-    const int K = a.D;
-    const size_t row = (size_t)i * K;
-    const float *z = a.z + row;
-    // softmax statistics of the row: lse of z (0 up to rounding, z being normalised)
-    double m = -INFINITY;
-    for (int k = lane; k < K; k += 32) m = fmax(m, (double)z[k]);
-    m = warp_max(m);
-    double s = 0.0;
-    for (int k = lane; k < K; k += 32) s += exp((double)z[k] - m);
-    const double lse = m + log(warp_sum(s));
-    // H = -sum p_j clamp(z_j)
-    double h = 0.0;
-    for (int k = lane; k < K; k += 32) {
-        const double p = exp((double)z[k] - lse);
-        h -= p * fmax((double)z[k], (double)-FLT_MAX);
-    }
-    h = warp_sum(h);
-    const int64_t act = a.act[i];
-    const bool valid = act >= 0 && act < K;
-    for (int k = lane; k < K; k += 32) {
-        const double zk = (double)z[k], p = exp(zk - lse);
-        const double dh = -p * ((zk >= (double)-FLT_MAX ? 1.0 : 0.0) + fmax(zk, (double)-FLT_MAX) + h);
-        double g = c_h * dh;
-        if (k == act) g += c_lp;
-        a.g_z[row + k] = valid ? (float)g : NAN;
-    }
+    const RowTerms t = categorical_row_grad(a, i, lane, c_lp, c_h);
     if (lane == 0) {
-        const double lp = valid ? (double)z[act] : NAN;
-        if (a.row_loss) a.row_loss[i] = (float)((-(double)a.R[i] * lp - (double)a.beta * h) * (double)a.inv_bs);
-        if (a.row_ent) a.row_ent[i] = (float)h;
+        if (a.row_loss) a.row_loss[i] = (float)((-(double)a.R[i] * t.lp - (double)a.beta * t.h) * (double)a.inv_bs);
+        if (a.row_ent) a.row_ent[i] = (float)t.h;
     }
 }
 
 __device__ void gaussian_row(const ReinforceArgs &a, int64_t i, int lane, double c_lp,
                              double c_h)
 {
-    const int A = a.D;
-    const size_t row = (size_t)i * A;
-    double lp = 0.0, h = 0.0;
-    for (int k = lane; k < A; k += 32) {
-        const double s = a.scale ? (double)a.scale[row + k] : 1.0;
-        const double d = (double)a.act_val[row + k] - (double)a.loc[row + k];
-        const double inv_s = 1.0 / s, ls = log(s);
-        a.g_loc[row + k] = (float)(c_lp * d * inv_s * inv_s);
-        if (a.g_scale)
-            a.g_scale[row + k] = (float)(c_lp * (d * d * inv_s * inv_s * inv_s - inv_s) + c_h * inv_s);
-        lp += -(d * d) * 0.5 * inv_s * inv_s - ls - kHalfLog2Pi;
-        h += 0.5 + kHalfLog2Pi + ls;
-    }
-    if (a.row_loss || a.row_ent) {
-        lp = warp_sum(lp);
-        h = warp_sum(h);
-        if (lane == 0) {
-            if (a.row_loss) a.row_loss[i] = (float)((-(double)a.R[i] * lp - (double)a.beta * h) * (double)a.inv_bs);
-            if (a.row_ent) a.row_ent[i] = (float)h;
-        }
+    const bool want = a.row_loss || a.row_ent;
+    const RowTerms t = gaussian_row_grad(a, i, lane, c_lp, c_h, want);
+    if (want && lane == 0) {
+        if (a.row_loss) a.row_loss[i] = (float)((-(double)a.R[i] * t.lp - (double)a.beta * t.h) * (double)a.inv_bs);
+        if (a.row_ent) a.row_ent[i] = (float)t.h;
     }
 }
 

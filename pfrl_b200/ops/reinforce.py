@@ -21,10 +21,12 @@ def _coefs(R, batchsize, beta):
     return c_lp.double(), float(c_h)
 
 
-def loss_grads_torch(R, batchsize, beta, *, z=None, actions=None, loc=None, scale=None,
-                     action_values=None, want_loss=False):
-    """The kernel's arithmetic in fp64 torch operations, stored in fp32."""
-    c_lp, c_h = _coefs(_f32(R).reshape(-1), batchsize, beta)
+def row_grads_torch(c_lp, c_h, *, z=None, actions=None, loc=None, scale=None,
+                    action_values=None):
+    """Given the gradients ``c_lp`` [N] (fp64) and ``c_h`` (a float) that a loss hands
+    log pi(a) and H of each row, the rows' d loss / d(distribution parameters) in fp64 torch
+    operations, stored in fp32: ``(grads, lp, h)`` with ``grads`` ``(g_z,)`` or
+    ``(g_loc, g_scale)`` and the rows' fp64 log pi(a) and H."""
     fmin = torch.finfo(torch.float32).min
     if z is not None:
         z = z.detach().double()
@@ -48,6 +50,15 @@ def loss_grads_torch(R, batchsize, beta, *, z=None, actions=None, loc=None, scal
         half_log_2pi = 0.5 * np.log(2 * np.pi)
         lp = (-(d * d) * 0.5 * inv_s * inv_s - s.log() - half_log_2pi).sum(1)
         h = (0.5 + half_log_2pi + s.log()).sum(1)
+    return out, lp, h
+
+
+def loss_grads_torch(R, batchsize, beta, *, z=None, actions=None, loc=None, scale=None,
+                     action_values=None, want_loss=False):
+    """The kernel's arithmetic in fp64 torch operations, stored in fp32."""
+    c_lp, c_h = _coefs(_f32(R).reshape(-1), batchsize, beta)
+    out, lp, h = row_grads_torch(c_lp, c_h, z=z, actions=actions, loc=loc, scale=scale,
+                                 action_values=action_values)
     if want_loss:
         Rd = _f32(R).reshape(-1).double()
         inv_bs = float(np.float32(1) / np.float32(batchsize))

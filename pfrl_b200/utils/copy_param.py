@@ -88,6 +88,24 @@ def copy_grad(target_link, source_link):
         dst.grad = None if src.grad is None else src.grad.clone()
 
 
+def copy_grad_into(target_link, source_link):
+    """``copy_grad``'s result, with the gradients that ``target_link`` already holds
+    overwritten in one multi-tensor copy instead of replaced by clones; a missing target
+    gradient is cloned once."""
+    dst, src = [], []
+    for t, s in zip(target_link.parameters(), source_link.parameters()):
+        assert t.shape == s.shape
+        if s.grad is None:
+            t.grad = None
+        elif t.grad is None or t.grad.dtype != s.grad.dtype or t.grad.device != s.grad.device:
+            t.grad = s.grad.clone()
+        else:
+            dst.append(t.grad)
+            src.append(s.grad)
+    if dst:
+        torch._foreach_copy_(dst, src)
+
+
 def synchronize_parameters(src, dst, method, tau=None):
     """copy_param.py:37-41"""
     if method == "hard":

@@ -19,7 +19,7 @@ from oracle.refimport import import_reference  # noqa: E402
 CALLABLES = """
 agents.DQN agents.DoubleDQN agents.CategoricalDQN agents.CategoricalDoubleDQN agents.IQN
 agents.AL agents.PAL agents.DoublePAL agents.DPP agents.dpp.DPPL agents.dpp.DPPGreedy
-agents.PPO agents.A2C agents.SoftActorCritic agents.TD3 agents.DDPG
+agents.PPO agents.A2C agents.SoftActorCritic agents.TD3 agents.DDPG agents.A3C
 replay_buffers.ReplayBuffer replay_buffers.PrioritizedReplayBuffer replay_buffers.EpisodicReplayBuffer
 nn.RecurrentSequential nn.RecurrentBranched replay_buffer.batch_recurrent_experiences
 replay_buffer.random_subseq replay_buffer.batch_experiences replay_buffer.ReplayUpdater utils.batch_states
