@@ -691,6 +691,36 @@ int b2rl_sac_target(const float *reward, const float *discount, const float *ter
                     const float *temperature_dev, float temperature, int32_t n,
                     float *out, void *stream);
 
+/* TD3's default target-policy smoothing (pfrl/agents/td3.py:20-24) for a given noise
+ * draw, n elements:
+ *   out = clamp(action + clamp(0.2 * noise, -0.5, 0.5), -1, 1)
+ * with one rounding per operation, as torch's eager sequence (clamp passes NaN through).
+ * The noise is the caller's torch.randn_like(action), so the random stream is the
+ * reference's.  0 < n < 2^39. */
+int b2rl_td3_smooth(const float *action, const float *noise, int64_t n, float *out,
+                    void *stream);
+
+/* The critic update of TD3 (pfrl/agents/td3.py:181-236) and DDPG
+ * (pfrl/agents/ddpg.py:150-173) after the forwards, in one launch, for n > 0 rows:
+ *   target  = reward + d * (1 - terminal) * next_q
+ *             (d = discount[i], the n-step discount of TD3, or gamma when discount is
+ *             NULL, as DDPG; next_q = torch.min(next_q1, next_q2), or next_q1 when
+ *             next_q2 is NULL), rounded like the reference's expression;
+ *   loss_c  = mse_loss(target, pred_c) with reduction "mean" (a deterministic fp32 sum in
+ *             an order of this kernel's own, divided by n);
+ *   grad_c  = float(2.0 / n) * (pred_c - target), rounded as torch's mse_loss backward,
+ *             which multiplies this by the upstream gradient.
+ * c = 1, and c = 2 when pred_q2 is not NULL (then grad2 and loss2 are required).
+ * A CTA takes B2RL_CRITIC_LOSS_ROWS_PER_CTA rows; when n exceeds that, `partial` must
+ * hold 2 * ceil(n / B2RL_CRITIC_LOSS_ROWS_PER_CTA) floats of scratch (else it may be
+ * NULL).  The call neither allocates nor synchronises. */
+#define B2RL_CRITIC_LOSS_ROWS_PER_CTA 1024
+int b2rl_td3_critic_loss(const float *reward, const float *discount, float gamma,
+                         const float *terminal, const float *next_q1, const float *next_q2,
+                         const float *pred_q1, const float *pred_q2, int32_t n, float *target,
+                         float *grad1, float *grad2, float *loss1, float *loss2,
+                         float *partial, void *stream);
+
 /* ------------------------------------------------------------------------
  * Dense contraction kept in exact fp32: first Nature-DQN convolution,
  * x[N,4,84,84] * w[32,4,8,8] (stride 4) + bias -> out[N,32,20,20].

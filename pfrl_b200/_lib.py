@@ -245,6 +245,9 @@ SIGNATURES = {
     "b2rl_a3c_loss": (_int, [_i64, _i32] + [_vp] * 8 + [_dbl] * 4 + [_vp] * 8),
     "b2rl_polyak": (_int, [ctypes.POINTER(TensorPair), _i32, _dbl, _vp]),
     "b2rl_sac_target": (_int, [_vp] * 7 + [ctypes.c_float, _i32, _vp, _vp]),
+    "b2rl_td3_smooth": (_int, [_vp, _vp, _i64, _vp, _vp]),
+    "b2rl_td3_critic_loss": (_int, [_vp, _vp, ctypes.c_float] + [_vp] * 5
+                             + [_i32] + [_vp] * 7),
     "b2rl_conv_nature1_fwd": (_int, [_vp, _vp, _vp, _i32, _vp, _vp]),
     "b2rl_conv_nature1_fwd_u8": (_int, [_vp, ctypes.c_float, _vp, _vp, _i32, _vp, _vp]),
     "b2rl_gemm_workspace_bytes": (_i64, [_i32, _i32, _i32]),

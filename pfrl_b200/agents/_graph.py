@@ -19,7 +19,10 @@ class CapturedStep:
     persistent buffers and returns them; ``run(fn)`` calls ``fn(buffers)`` eagerly ``warmup``
     times, then captures one call and from then on replays it and returns the captured
     outputs.  With ``share_pool_with``, the graph is captured into that step's memory pool;
-    the two must then replay in the order they were captured.
+    the two must then replay in the order they were captured.  With ``pool`` (a
+    ``torch.cuda.graph_pool_handle()``), it is captured into that pool, which several steps
+    can share whichever of them captures first; such steps must replay one after another on
+    one stream, each one's outputs consumed before another replays.
 
     A capture bakes in the addresses of the tensors the call reads and every Python number
     it reads: an optimizer's scalar ``lr``, a loss coefficient handed to a kernel.  So the
@@ -30,11 +33,12 @@ class CapturedStep:
     and that no hook changes (C51's atoms, IQN's quantile counts, the α and η of AL and DPP)
     are left out.  A changed key drops the graph: the call warms up and is captured again."""
 
-    def __init__(self, warmup, optimizers=(), share_pool_with=None):
+    def __init__(self, warmup, optimizers=(), share_pool_with=None, pool=None):
         self.warmup = warmup
         self.optimizers = [opt for opt in optimizers if opt is not None]
         make_capturable(*self.optimizers)
         self.share_pool_with = share_pool_with
+        self.pool = pool
         self.key = self.graph = None
 
     def load(self, key, inputs):
@@ -56,7 +60,7 @@ class CapturedStep:
             if self.warm < self.warmup:  # optimizer state, cuBLAS / cuDNN plans
                 self.warm += 1
                 return fn(self.buffers)
-            pool = self.share_pool_with.graph.pool() if self.share_pool_with else None
+            pool = self.share_pool_with.graph.pool() if self.share_pool_with else self.pool
             self.graph = torch.cuda.CUDAGraph()
             # torch.cuda.graph synchronises the device before it captures
             with no_distribution_validation(), torch.cuda.graph(self.graph, pool=pool):

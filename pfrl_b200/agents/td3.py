@@ -6,7 +6,18 @@ SAC unchanged; only the update differs.  Public surface as in the reference
 arguments, saved_attributes, statistics names.  Statistics stay on the device
 (no per-update ``.item()`` / ``.cpu()`` as in td3.py:217-220,237) and the
 Polyak steps are multi-tensor launches.
+
+On CUDA with fp32 critics (``use_fused``, on by default) the critic update's tail runs in
+csrc/sac.cu: TD3's default target-policy smoothing (``k_td3_smooth``, on the reference's
+``torch.randn_like`` draw) and, in one launch, the target, both critics' ``mse_loss`` and
+their gradients (``k_td3_critic_loss``).  The forwards keep the reference's order, so the
+random stream is the reference's.  The fused update runs with the distributions' argument
+checks off (each is a host sync), so an update on the device replay path does not wait for
+the device.  ``cuda_graph=True`` replays each update as a CUDA graph: TD3 has two, the
+critic-only update and the critic + policy + Polyak update, in one memory pool; DDPG has
+one, critic and actor (its target sync stays in ``_on_step``).
 """
+import contextlib
 import copy
 from logging import getLogger
 
@@ -15,12 +26,14 @@ from torch import nn
 from torch.nn import functional as F
 
 from pfrl_b200.agent import AttributeSavingMixin, BatchAgent
+from pfrl_b200.agents._graph import CapturedStep
 from pfrl_b200.agents.dqn import _DeviceRing
+from pfrl_b200.ops import sac as sac_ops
 from pfrl_b200.replay_buffer import ReplayUpdater, batch_experiences
 from pfrl_b200.utils import clip_l2_grad_norm_
 from pfrl_b200.utils.batch_states import batch_states
 from pfrl_b200.utils.copy_param import synchronize_parameters
-from pfrl_b200.utils.modes import evaluating
+from pfrl_b200.utils.modes import evaluating, no_distribution_validation
 
 
 def default_target_policy_smoothing_func(batch_action):
@@ -94,6 +107,17 @@ class _OffPolicyActorCritic(AttributeSavingMixin, BatchAgent):
     def _on_step(self):
         pass
 
+    # the batch entries a graphed update reads
+    _GRAPH_KEYS = ("state", "next_state", "action", "reward", "discount", "is_state_terminal")
+
+    def _fused(self, *tensors):
+        return self.use_fused and all(t.is_cuda and t.dtype == torch.float32 for t in tensors)
+
+    def _update_context(self):
+        """No distribution argument checks (a host sync each) in a fused update."""
+        fused = self.use_fused and self.device.type == "cuda"
+        return no_distribution_validation() if fused else contextlib.nullcontext()
+
     def _opt_step(self, optimizer, module, loss, max_grad_norm=None):
         optimizer.zero_grad()
         loss.backward()
@@ -103,6 +127,7 @@ class _OffPolicyActorCritic(AttributeSavingMixin, BatchAgent):
 
 
 class TD3(_OffPolicyActorCritic):
+    use_fused = True
     saved_attributes = (
         "policy", "q_func1", "q_func2", "target_policy", "target_q_func1", "target_q_func2",
         "policy_optimizer", "q_func1_optimizer", "q_func2_optimizer",
@@ -114,7 +139,8 @@ class TD3(_OffPolicyActorCritic):
                  phi=lambda x: x, soft_update_tau=5e-3, n_times_update=1, max_grad_norm=None,
                  logger=getLogger(__name__), batch_states=batch_states, burnin_action_func=None,
                  policy_update_delay=2,
-                 target_policy_smoothing_func=default_target_policy_smoothing_func):
+                 target_policy_smoothing_func=default_target_policy_smoothing_func,
+                 cuda_graph=False):
         self._init_common(policy, replay_buffer, gamma, explorer, gpu, phi, batch_states,
                           burnin_action_func, logger)
         self.policy, self.q_func1, self.q_func2 = policy, q_func1, q_func2
@@ -142,6 +168,14 @@ class TD3(_OffPolicyActorCritic):
         self.q_func1_loss_record = _DeviceRing(100)
         self.q_func2_loss_record = _DeviceRing(100)
         self.policy_loss_record = _DeviceRing(100)
+        # cuda_graph=True: the critic-only update and the critic + policy + Polyak update,
+        # captured into one memory pool
+        self._q_graph = self._full_graph = None
+        if cuda_graph and self.device.type == "cuda":
+            pool = torch.cuda.graph_pool_handle()
+            self._q_graph = CapturedStep(3, (q_func1_optimizer, q_func2_optimizer), pool=pool)
+            self._full_graph = CapturedStep(
+                3, (q_func1_optimizer, q_func2_optimizer, policy_optimizer), pool=pool)
 
     def _n_policy_updates(self):
         return self.policy_n_updates
@@ -151,44 +185,92 @@ class TD3(_OffPolicyActorCritic):
                          (self.q_func2, self.target_q_func2)):
             synchronize_parameters(src=src, dst=dst, method="soft", tau=self.soft_update_tau)
 
-    def update_q_func(self, batch):
-        """Clipped double-Q regression with target policy smoothing (td3.py:181-236)."""
+    def _smooth(self, next_actions):
+        if (self.target_policy_smoothing_func is default_target_policy_smoothing_func
+                and self._fused(next_actions)):
+            return sac_ops.td3_smooth(next_actions, torch.randn_like(next_actions))
+        return self.target_policy_smoothing_func(next_actions)
+
+    def _q_step(self, batch):
+        """The device work of update_q_func; returns the predictions and the losses."""
         next_state = batch["next_state"]
         with torch.no_grad(), evaluating(self.target_policy), evaluating(self.target_q_func1), \
                 evaluating(self.target_q_func2):
-            next_actions = self.target_policy_smoothing_func(
-                self.target_policy(next_state).sample())
-            next_q = torch.min(self.target_q_func1((next_state, next_actions)),
-                               self.target_q_func2((next_state, next_actions)))
-            target_q = batch["reward"] + batch["discount"] * (
-                1.0 - batch["is_state_terminal"]) * torch.flatten(next_q)
+            next_actions = self._smooth(self.target_policy(next_state).sample())
+            next_q1 = self.target_q_func1((next_state, next_actions))
+            next_q2 = self.target_q_func2((next_state, next_actions))
         state, actions = batch["state"], batch["action"]
         predict_q1 = torch.flatten(self.q_func1((state, actions)))
         predict_q2 = torch.flatten(self.q_func2((state, actions)))
-        loss1 = F.mse_loss(target_q, predict_q1)
-        loss2 = F.mse_loss(target_q, predict_q2)
-        self.q1_record.extend(predict_q1)
-        self.q2_record.extend(predict_q2)
-        self.q_func1_loss_record.append(loss1.detach())
-        self.q_func2_loss_record.append(loss2.detach())
+        if self._fused(next_q1, next_q2, predict_q1, predict_q2):
+            _, loss1, loss2 = sac_ops.critic_loss(
+                batch["reward"], batch["discount"], batch["is_state_terminal"], next_q1, next_q2,
+                predict_q1, predict_q2)
+        else:
+            with torch.no_grad():
+                next_q = torch.min(next_q1, next_q2)
+                target_q = batch["reward"] + batch["discount"] * (
+                    1.0 - batch["is_state_terminal"]) * torch.flatten(next_q)
+            loss1 = F.mse_loss(target_q, predict_q1)
+            loss2 = F.mse_loss(target_q, predict_q2)
         self._opt_step(self.q_func1_optimizer, self.q_func1, loss1, self.max_grad_norm)
         self._opt_step(self.q_func2_optimizer, self.q_func2, loss2, self.max_grad_norm)
+        return predict_q1.detach(), predict_q2.detach(), loss1.detach(), loss2.detach()
+
+    def _record_q_step(self, q1, q2, loss1, loss2):
+        self.q1_record.extend(q1)
+        self.q2_record.extend(q2)
+        self.q_func1_loss_record.append(loss1)
+        self.q_func2_loss_record.append(loss2)
         self.q_func_n_updates += 1
 
-    def update_policy(self, batch):
+    def update_q_func(self, batch):
+        """Clipped double-Q regression with target policy smoothing (td3.py:181-236)."""
+        self._record_q_step(*self._q_step(batch))
+
+    def _policy_step(self, batch):
         state = batch["state"]
         q = self.q_func1((state, self.policy(state).rsample()))
         loss = -torch.mean(q)
-        self.policy_loss_record.append(loss.detach())
         self._opt_step(self.policy_optimizer, self.policy, loss, self.max_grad_norm)
+        return loss.detach()
+
+    def _record_policy_step(self, loss):
+        self.policy_loss_record.append(loss)
         self.policy_n_updates += 1
+
+    def update_policy(self, batch):
+        self._record_policy_step(self._policy_step(batch))
+
+    def _graphed_update(self, batch):
+        policy = (self.q_func_n_updates + 1) % self.policy_update_delay == 0
+        step = self._full_graph if policy else self._q_graph
+        step.load((self.soft_update_tau, self.max_grad_norm, self.policy_update_delay,
+                   self.target_policy_smoothing_func, self.use_fused),
+                  {k: batch[k] for k in self._GRAPH_KEYS})
+
+        def core(b):
+            out = self._q_step(b)
+            if policy:
+                out += (self._policy_step(b),)
+                self.sync_target_network()
+            return out
+
+        out = step.run(core)
+        self._record_q_step(*out[:4])
+        if policy:
+            self._record_policy_step(out[4])
 
     def update(self, experiences, errors_out=None):
         batch = batch_experiences(experiences, self.device, self.phi, self.gamma)
-        self.update_q_func(batch)
-        if self.q_func_n_updates % self.policy_update_delay == 0:
-            self.update_policy(batch)
-            self.sync_target_network()
+        with self._update_context():
+            if self._q_graph is not None:
+                self._graphed_update(batch)
+                return
+            self.update_q_func(batch)
+            if self.q_func_n_updates % self.policy_update_delay == 0:
+                self.update_policy(batch)
+                self.sync_target_network()
 
     def get_statistics(self):
         return [
@@ -203,6 +285,7 @@ class TD3(_OffPolicyActorCritic):
 
 
 class DDPG(_OffPolicyActorCritic):
+    use_fused = True
     saved_attributes = ("model", "target_model", "actor_optimizer", "critic_optimizer")
 
     def __init__(self, policy, q_func, actor_optimizer, critic_optimizer, replay_buffer, gamma,
@@ -210,7 +293,7 @@ class DDPG(_OffPolicyActorCritic):
                  update_interval=1, target_update_interval=10000, phi=lambda x: x,
                  target_update_method="hard", soft_update_tau=1e-2, n_times_update=1,
                  recurrent=False, episodic_update_len=None, logger=getLogger(__name__),
-                 batch_states=batch_states, burnin_action_func=None):
+                 batch_states=batch_states, burnin_action_func=None, cuda_graph=False):
         assert not recurrent, "recurrent=True is not implemented"
         self._init_common(policy, replay_buffer, gamma, explorer, gpu, phi, batch_states,
                           burnin_action_func, logger)
@@ -235,6 +318,10 @@ class DDPG(_OffPolicyActorCritic):
         self.policy, self.q_function = self.model
         self.target_policy, self.target_q_function = self.target_model
         self.sync_target_network()
+        # cuda_graph=True: the critic and actor steps as one graph
+        self._graph = None
+        if cuda_graph and self.device.type == "cuda":
+            self._graph = CapturedStep(3, (critic_optimizer, actor_optimizer))
 
     def _n_policy_updates(self):
         return self.n_updates
@@ -247,35 +334,65 @@ class DDPG(_OffPolicyActorCritic):
         synchronize_parameters(src=self.model, dst=self.target_model,
                                method=self.target_update_method, tau=self.soft_update_tau)
 
-    def compute_critic_loss(self, batch):
-        """1-step TD regression; note gamma, not the n-step discount (ddpg.py:150-173)."""
+    def _critic_loss(self, batch):
         n = len(batch["reward"])
         with torch.no_grad():
             next_state = batch["next_state"]
             next_q = self.target_q_function((next_state, self.target_policy(next_state).sample()))
+        predict_q = self.q_function((batch["state"], batch["action"])).reshape((n,))
+        if self._fused(next_q, predict_q):
+            return sac_ops.critic_loss(batch["reward"], self.gamma, batch["is_state_terminal"],
+                                       next_q, None, predict_q, None)[1]
+        with torch.no_grad():
             target_q = batch["reward"] + self.gamma * (
                 1.0 - batch["is_state_terminal"]) * next_q.reshape((n,))
-        predict_q = self.q_function((batch["state"], batch["action"])).reshape((n,))
-        loss = F.mse_loss(target_q, predict_q)
+        return F.mse_loss(target_q, predict_q)
+
+    def compute_critic_loss(self, batch):
+        """1-step TD regression; note gamma, not the n-step discount (ddpg.py:150-173)."""
+        loss = self._critic_loss(batch)
         self.critic_loss_record.append(loss.detach())
         return loss
 
-    def compute_actor_loss(self, batch):
+    def _actor_loss(self, batch):
         state = batch["state"]
         q = self.q_function((state, self.policy(state).rsample()))
-        loss = -q.mean()
+        return -q.mean(), q
+
+    def compute_actor_loss(self, batch):
+        loss, q = self._actor_loss(batch)
         self.q_record.extend(q)
         self.actor_loss_record.append(loss.detach())
         return loss
 
-    def update(self, experiences, errors_out=None):
-        batch = batch_experiences(experiences, self.device, self.phi, self.gamma)
+    def _graph_step(self, batch):
         self.critic_optimizer.zero_grad()
-        self.compute_critic_loss(batch).backward()
+        critic_loss = self._critic_loss(batch)
+        critic_loss.backward()
         self.critic_optimizer.step()
         self.actor_optimizer.zero_grad()
-        self.compute_actor_loss(batch).backward()
+        actor_loss, q = self._actor_loss(batch)
+        actor_loss.backward()
         self.actor_optimizer.step()
+        return critic_loss.detach(), actor_loss.detach(), q.detach()
+
+    def update(self, experiences, errors_out=None):
+        batch = batch_experiences(experiences, self.device, self.phi, self.gamma)
+        with self._update_context():
+            if self._graph is not None:
+                self._graph.load((self.gamma, self.use_fused),
+                                 {k: batch[k] for k in self._GRAPH_KEYS})
+                critic_loss, actor_loss, q = self._graph.run(self._graph_step)
+                self.critic_loss_record.append(critic_loss)
+                self.q_record.extend(q)
+                self.actor_loss_record.append(actor_loss)
+            else:
+                self.critic_optimizer.zero_grad()
+                self.compute_critic_loss(batch).backward()
+                self.critic_optimizer.step()
+                self.actor_optimizer.zero_grad()
+                self.compute_actor_loss(batch).backward()
+                self.actor_optimizer.step()
         self.n_updates += 1
 
     def get_statistics(self):
