@@ -481,13 +481,14 @@ class ACER(agent.AttributeSavingMixin, agent.AsyncAgent):
     def _replay_inputs(self, episodes):
         """(states [T(+1), ...], actions [T], rewards fp64 [T], mu logits [T, K], terminal)
         of the one sampled subsequence, on the device; None where the buffer cannot give
-        them (a mu that is not a Categorical)."""
+        them (a mu that is not an fp32 Categorical)."""
         from pfrl_b200.replay_buffers.episodic import DeviceEpisodes
 
         dev = self.device
         if isinstance(episodes, DeviceEpisodes):
             rbuf = episodes.buffer
-            if rbuf._mu_layout is None or rbuf._mu_layout[0] is not torch.distributions.Categorical:
+            if (rbuf._mu_layout is None or rbuf._mu_layout[0] is not torch.distributions.Categorical
+                    or rbuf._mu_layout[2] != torch.float32):
                 return None
             terminal = bool(episodes.last_terminal[0])
             batch = rbuf._gather_sequences(episodes, 1.0, self.phi)

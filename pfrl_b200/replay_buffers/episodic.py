@@ -17,13 +17,15 @@ observations and records live in the part ring and record store of
     by any live episode or any uncommitted current episode;
   * a recurrent-state ring in HBM: ``recurrent_state`` / ``next_recurrent_state``
     of every transition (device tensors, numpy arrays or None; any nesting of
-    tuples) flattened to one fp32 row each, at row ``absolute index % capacity``;
+    tuples) flattened to one row of fp32 words each, at row ``absolute index % capacity``.
+    A leaf keeps the dtype it was appended in: 4- and 8-byte types are stored as their
+    bits, fp16 widened to fp32, and both come back unchanged;
   * a behaviour-policy ring in HBM for ACER: the ``mu`` distribution appended with a
-    transition, as one fp32 row at the same row index (a ``Categorical``'s normalised
-    logits [K], or an ``Independent(Normal, 1)``'s loc and scale [2A]).  The first
-    ``mu`` fixes the layout.  The host episode table also records which episodes
-    ended on a terminal, so a sampled subsequence's last transition is known to be
-    terminal or not without reading the device.
+    transition, as one row at the same row index, in the distribution's dtype (a
+    ``Categorical``'s normalised logits [K], or an ``Independent(Normal, 1)``'s loc and
+    scale [2A]).  The first ``mu`` fixes the layout.  The host episode table also
+    records which episodes ended on a terminal, so a sampled subsequence's last
+    transition is known to be terminal or not without reading the device.
 
 ``sample_episodes`` returns ``DeviceEpisodes``; ``batch_recurrent_experiences``
 turns it into the packed minibatch with one kernel launch
@@ -127,15 +129,16 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
         self._ep_count = 0                     # episodes ever committed
         self._min_seq = collections.deque()    # (episode number, seq): sliding-window minimum
         self._rs_struct = None                 # structure of the first non-None state
-        self._rs_leaves = None                 # [(offset, d0, inner)] per leaf
-        self._rs_ring = None                   # [alloc, 2, D] fp32 (HBM)
+        self._rs_dtypes = None                 # appended dtype of every leaf
+        self._rs_leaves = None                 # [(offset, d0, inner)] per leaf, in fp32 words
+        self._rs_ring = None                   # [alloc, 2, D] fp32 words (HBM)
         self._rs_present = None                # [alloc, 2] uint8 (HBM)
         self._rs_present_host = None           # host mirror of _rs_present
         self._pend_rs = []                     # (ring row * 2 + side, flat row or None)
         self._current_mu = collections.defaultdict(list)  # env_id -> [mu row or None]
         self._terminal_ends = set()            # abs end of the live episodes ending terminal
-        self._mu_layout = None                 # (distribution class, width) of the first mu
-        self._mu_ring = None                   # [alloc, width] fp32 (HBM)
+        self._mu_layout = None                 # (distribution class, width, dtype) of the first mu
+        self._mu_ring = None                   # [alloc, width] in that dtype (HBM)
         self._mu_present_host = None           # [alloc] bool
         self._pend_mu = []                     # (ring row, mu row or None)
 
@@ -158,10 +161,12 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
             n_slots, n_min = self._parts_of(next_state)
         rec = (s_slots, self.layout._action_array(action).tobytes(), float(reward), n_slots,
                bool(is_state_terminal), min(s_min, n_min))
+        # everything that can refuse the transition runs before any of it is kept
         rs = self._flat_state(kwargs.get("recurrent_state"))
         nrs = self._flat_state(kwargs.get("next_recurrent_state"))
+        mu = self._flat_mu(kwargs.get("mu"))
         self.current_episode[env_id].append((rec, rs, nrs))
-        self._current_mu[env_id].append(self._flat_mu(kwargs.get("mu")))
+        self._current_mu[env_id].append(mu)
         if is_state_terminal:
             self.stop_current_episode(env_id=env_id)
 
@@ -283,24 +288,29 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
     def _flat_state(self, state):
         if state is None:
             return None
-        leaves = _leaves(state)
+        leaves = [x.detach() if isinstance(x, torch.Tensor)
+                  else torch.from_numpy(np.ascontiguousarray(x)) for x in _leaves(state)]
+        dtypes = tuple(x.dtype for x in leaves)
         if self._rs_struct is None:
-            self._rs_struct = _structure(state)
             specs, off = [], 0
             for x in leaves:
                 shape = tuple(x.shape)
                 assert len(shape) >= 1, "recurrent state tensors need at least one axis"
                 inner = int(np.prod(shape[1:])) if len(shape) > 1 else 1
+                inner *= _state_words(x.dtype)
                 specs.append((off, shape[0], inner))
                 off += shape[0] * inner
             assert len(specs) <= _lib.SEQ_MAX_LEAVES
+            self._rs_struct = _structure(state)
+            self._rs_dtypes = dtypes
             self._rs_leaves = specs
             self._rs_width = off
         assert _structure(state) == self._rs_struct, "recurrent state layout changed"
-        parts = [x.detach().reshape(-1) if isinstance(x, torch.Tensor)
-                 else torch.from_numpy(np.ascontiguousarray(x).reshape(-1)) for x in leaves]
-        row = parts[0] if len(parts) == 1 else torch.cat(parts)
-        return row.float() if row.dtype != torch.float32 else row
+        if dtypes != self._rs_dtypes:
+            raise TypeError("recurrent state dtypes changed: %s, the buffer holds %s"
+                            % (dtypes, self._rs_dtypes))
+        parts = [_state_to_words(x).reshape(-1) for x in leaves]
+        return parts[0] if len(parts) == 1 else torch.cat(parts)
 
     def _flush_states(self):
         pend = self._pend_rs
@@ -332,7 +342,7 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
 
     # -- behaviour policies (ACER's mu) -------------------------------------------
     def _flat_mu(self, mu):
-        """One fp32 row of ``mu`` (a device or host tensor; no copy to the host)."""
+        """One row of ``mu`` in its dtype (a device or host tensor; no copy to the host)."""
         if mu is None:
             return None
         D = torch.distributions
@@ -346,13 +356,14 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
             raise NotImplementedError(
                 "EpisodicReplayBuffer stores mu as a Categorical or an Independent(Normal, 1) "
                 "distribution, got %s" % type(mu).__name__)
-        layout = (type(mu), int(row.numel()))
+        layout = (type(mu), int(row.numel()), row.dtype)
         if self._mu_layout is None:
             self._mu_layout = layout
         assert layout == self._mu_layout, \
-            "mu layout changed: %s of width %d, the buffer holds %s of width %d" % (
-                layout[0].__name__, layout[1], self._mu_layout[0].__name__, self._mu_layout[1])
-        return row.float() if row.dtype != torch.float32 else row
+            "mu layout changed: %s of width %d (%s), the buffer holds %s of width %d (%s)" % (
+                layout[0].__name__, layout[1], layout[2], self._mu_layout[0].__name__,
+                self._mu_layout[1], self._mu_layout[2])
+        return row
 
     def _flush_mu(self):
         pend = self._pend_mu
@@ -362,7 +373,7 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
         dev = self.device
         if self._mu_ring is None:
             self._mu_ring = torch.zeros((self._alloc_capacity, self._mu_layout[1]),
-                                        dtype=torch.float32, device=dev)
+                                        dtype=self._mu_layout[2], device=dev)
             self._mu_present_host = np.zeros(self._alloc_capacity, dtype=bool)
         # only the last write of a ring row may reach the scatter
         pend = list({k: (k, r) for k, r in pend}.values())
@@ -375,7 +386,7 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
 
     def _mu_distribution(self, row):
         """``row`` [width] rebuilt as the stored class with a batch axis of 1."""
-        cls, width = self._mu_layout
+        cls, width, _ = self._mu_layout
         if cls is torch.distributions.Categorical:
             return cls(logits=row[None])
         A = width // 2
@@ -475,7 +486,9 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
             for key, leaves in (("recurrent_state", out["state_leaves"]),
                                 ("next_recurrent_state", out["next_state_leaves"])):
                 shaped = []
-                for x, shape in zip(leaves, _leaves_of_structure(self._rs_struct)):
+                for x, dt, shape in zip(leaves, self._rs_dtypes,
+                                        _leaves_of_structure(self._rs_struct)):
+                    x = _state_from_words(x, dt)  # [d0, B, inner words] -> appended dtype
                     shaped.append(x.view((shape[0], B) + tuple(shape[1:])))
                 batch[key] = _rebuild(self._rs_struct, shaped)
             # a sequence whose first state was stored as None gets zeros, as
@@ -560,7 +573,10 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
         if self._rs_ring is None:
             return [(None, None)] * len(absolute)
         rows = np.asarray(absolute, dtype=np.int64) % self._alloc_capacity
-        flat = self._rs_ring[torch.as_tensor(rows).to(self.device)].cpu().numpy()
+        flat = self._rs_ring[torch.as_tensor(rows).to(self.device)].cpu()
+        # every leaf of every row, back in its appended dtype: [rows, 2, elements]
+        cols = [_state_from_words(flat[:, :, off:off + d0 * inner], dt).numpy()
+                for (off, d0, inner), dt in zip(self._rs_leaves, self._rs_dtypes)]
         present = self._rs_present_host[rows]
         shapes = _leaves_of_structure(self._rs_struct)
         out = []
@@ -570,8 +586,7 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
                 if not present[i, side]:
                     pair.append(None)
                     continue
-                leaves = [flat[i, side, off:off + d0 * inner].reshape(shape)
-                          for (off, d0, inner), shape in zip(self._rs_leaves, shapes)]
+                leaves = [c[i, side].reshape(shape) for c, shape in zip(cols, shapes)]
                 pair.append(_rebuild(self._rs_struct, leaves))
             out.append(tuple(pair))
         return out
@@ -589,6 +604,35 @@ class EpisodicReplayBuffer(DeviceNStepBuffer):
             out.extend(self._materialise_episodes(
                 DeviceEpisodes(self, eps.first[sl], eps.length[sl], eps.end[sl])))
         return out
+
+
+def _state_words(dtype):
+    """fp32 words per element of a recurrent-state leaf of ``dtype`` in the ring: 4- and
+    8-byte types are stored as their bits, fp16 widened to fp32 (exact both ways)."""
+    if dtype == torch.float16:
+        return 1
+    size = torch.empty(0, dtype=dtype).element_size()
+    if size not in (4, 8) or dtype.is_complex:
+        raise TypeError("EpisodicReplayBuffer stores recurrent states of 4- or 8-byte dtypes "
+                        "or float16, got %s" % dtype)
+    return size // 4
+
+
+def _state_to_words(x):
+    if x.dtype == torch.float32:
+        return x
+    if x.dtype == torch.float16:
+        return x.float()
+    return x.contiguous().view(torch.float32)  # the bits, word by word
+
+
+def _state_from_words(x, dtype):
+    """``x`` [..., words] fp32 back to ``dtype`` [..., elements]."""
+    if dtype == torch.float32:
+        return x
+    if dtype == torch.float16:
+        return x.to(dtype)
+    return x.contiguous().view(dtype)
 
 
 def _leaves_of_structure(structure):
